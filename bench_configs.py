@@ -4,11 +4,12 @@
   config 1: the reference's own elembench (cli/Benchmark.cpp, unmodified) on the plumbing graph, against both engines
   config 3: additive synth, 64 el.cycle partials per voice (387 nodes)          — K1, many recurrences per voice
   config 4: el.convolve reverb, 16384-tap IR, one channel per voice             — K3 (partitioned FFT convolver)
+  config 4v: the same with a different 16384-tap IR on every channel           — K3, per-channel-IR form (not in the default set)
   config 5: independent random 64-node graphs, one voice group each             — K1, one launch per graph
 
 Each prints one JSON line: device-resident ms/block (CUDA events), Msamples/s, x real time, the kernel time measured
 with events around the K1/K3 launches, the algorithmic-bytes roofline fraction and a CPU reference sample
-(unmodified reference via oracle/_ref on all host threads).  Usage: python bench_configs.py [1] [3] [4] [5] [--quick]
+(unmodified reference via oracle/_ref on all host threads).  Usage: python bench_configs.py [1] [3] [4] [4v] [5] [--quick]
 """
 from __future__ import annotations
 
@@ -132,6 +133,86 @@ def config4(quick, steps=None):
             "launches_per_block": launches, "cpu_reference": cpu}
 
 
+def config4v(quick, steps=None):
+    """BASELINE config 4's per-channel-IR variant: 1024 channels, each with its own 16384-tap IR (Runtime.set_path_per_voice: one
+    voice group, the per-channel form of K3), parity of 8 sampled channels against the reference over 40 blocks, and for contrast
+    the same workload at 128 channels through per-voice JSON `path` batches (every voice its own group and K3 launch)."""
+    import torch
+    from bench import gpu_description
+    from oracle import oracle as orc
+    from elementary_b200 import Runtime, el, graphs
+    from elementary_b200.runtime import FLAG_MIX, FLAG_VOICE_IN
+    channels = 1024
+    t0 = time.perf_counter()
+    irs = [np.asarray(graphs.lcg_ir(16384, seed=c + 1), dtype=np.float32) for c in range(channels)]
+    gen_s = time.perf_counter() - t0
+    names = [f"ir{c}" for c in range(channels)]
+    cv = el.convolve({"path": names[0], "key": "cv"}, el.in_(0))
+    batch = el.render(cv)
+    t0 = time.perf_counter()
+    rt = Runtime(SR, BS, channels, device=0, time_kernels=1)
+    for nm, ir in zip(names, irs):
+        assert rt.add_shared_resource(nm, ir)
+    assert rt.apply_instructions(batch) == 0, rt.last_error()
+    assert rt.set_path_per_voice(cv.id(), names, np.arange(channels)) == 0, rt.last_error()
+    rt.synchronize()
+    setup_s = time.perf_counter() - t0
+    desc = rt.describe()
+    assert len(desc["groups"]) == 1 and desc["groups"][0]["convolvers"][0]["form"] == "per_channel"
+
+    # parity first (host I/O, 40 blocks from silence), then a fresh runtime for the device-resident timing
+    nb = 40
+    sample = np.random.RandomState(1).choice(channels, size=8, replace=False)
+    x = ((np.random.RandomState(2).rand(channels, 1, nb * BS) - 0.5) * 0.5).astype(np.float32)
+    got, _ = rt.render_voices(nb, 1, x)
+    parity = {"available": orc.ref_available(), "channels": [int(c) for c in sample], "blocks": nb}
+    if orc.ref_available():
+        worst = 0.0
+        for c in sample:
+            o = orc.RefRuntime(SR, BS)
+            assert o.add_shared_resource(names[c], irs[c]) and o.apply(el.render(el.convolve({"path": names[c], "key": "cv"}, el.in_(0)))) == 0
+            ref = o.render(nb, 1, BS, x[c])
+            worst = max(worst, float(np.abs(got[c].astype(np.float64) - ref).max() / np.abs(ref).max()))
+        parity.update({"worst_err_over_peak": worst, "ok": worst <= 1e-5})
+    del rt
+
+    rt = Runtime(SR, BS, channels, device=0, time_kernels=1)
+    for nm, ir in zip(names, irs):
+        rt.add_shared_resource(nm, ir)
+    assert rt.apply_instructions(batch) == 0 and rt.set_path_per_voice(cv.id(), names, np.arange(channels)) == 0
+    xd = torch.as_tensor(rt.voice_in_device(1), device="cuda")
+    xd.copy_((torch.rand(xd.shape, device="cuda") - 0.5) * 0.5)
+    ms, k1, k3, launches = timed_blocks(rt, 1, FLAG_MIX | FLAG_VOICE_IN, steps or (10 if quick else 60), 40)
+    S = 32
+    today = 2 * 512 * 4 + (S - 1) * 513 * 8 + 513 * 8 + 2 * 512 * 4          # config 4's formula
+    algo = (today + S * 4096) * channels                                      # + every channel's own IR spectra (no unit shares an IR)
+    del rt
+
+    # contrast: per-voice JSON `path` batches cut the group into one group (one K3 launch) per voice
+    n_json = 128
+    t0 = time.perf_counter()
+    rj = Runtime(SR, BS, n_json, device=0, time_kernels=1)
+    for nm, ir in zip(names[:n_json], irs[:n_json]):
+        rj.add_shared_resource(nm, ir)
+    assert rj.apply_instructions(batch) == 0
+    for v in range(1, n_json):
+        assert rj.apply_instructions([[3, cv.id(), "path", names[v]]], voices=(v, v + 1)) == 0, rj.last_error()
+    rj.synchronize()
+    json_setup_s = time.perf_counter() - t0
+    xj = torch.as_tensor(rj.voice_in_device(1), device="cuda")
+    xj.copy_((torch.rand(xj.shape, device="cuda") - 0.5) * 0.5)
+    jms, _, jk3, jl = timed_blocks(rj, 1, FLAG_MIX | FLAG_VOICE_IN, steps or (10 if quick else 30), 40)
+    contrast = {"channels": n_json, "groups": len(rj.describe()["groups"]), "ms_per_block": jms, "k3_ms": jk3, "launches_per_block": jl,
+                "setup_s": json_setup_s}
+    del rj
+    return {"config": "4v: el.convolve, 1024 channels each with its own 16384-tap IR (set_path_per_voice), one GPU",
+            "ms_per_block": ms, "k1_ms": k1, "k3_ms": k3, "launches_per_block": launches,
+            "setup_s": setup_s, "ir_generation_s": gen_s,
+            "roofline": {"bound": "hbm", "kernel": "convolve_chunk_tm_kernel<per-channel>", "achieved_gbs": algo / (k3 * 1e-3) / 1e9,
+                         "peak_gbs": hbm_peak(), "frac": algo / (k3 * 1e-3) / 1e9 / hbm_peak(), "algorithmic_bytes_per_channel_block": algo // channels},
+            "gpu": gpu_description(0), "parity": parity, "json_per_voice_paths": contrast}
+
+
 def config5(quick, steps=None):
     from elementary_b200 import Runtime, graphs
     from elementary_b200.runtime import FLAG_MIX
@@ -198,9 +279,9 @@ def config5(quick, steps=None):
 
 def main():
     quick = "--quick" in sys.argv
-    which = [a for i, a in enumerate(sys.argv[1:], 1) if a in ("1", "3", "4", "5") and sys.argv[i - 1] not in ("--stages", "--graphs", "--niter", "--wpc")] or ["1", "3", "4", "5"]
+    which = [a for i, a in enumerate(sys.argv[1:], 1) if a in ("1", "3", "4", "4v", "5") and sys.argv[i - 1] not in ("--stages", "--graphs", "--niter", "--wpc")] or ["1", "3", "4", "5"]
     for w in which:
-        r = {"1": config1, "3": config3, "4": config4, "5": config5}[w](quick)
+        r = {"1": config1, "3": config3, "4": config4, "4v": config4v, "5": config5}[w](quick)
         print(json.dumps(r))
         sys.stdout.flush()
 

@@ -75,6 +75,11 @@ int elem_b200_set_property_per_voice(elem_b200_runtime* rt, int32_t nodeId, cons
     GUARD(rt->engine->setPropertyPerVoice(nodeId, key, values, voiceBegin, count));
 }
 
+int elem_b200_set_path_per_voice(elem_b200_runtime* rt, int32_t nodeId, const char* const* names, int numNames, const int32_t* index, int voiceBegin, int count) {
+    if ((numNames > 0 && !names) || (count > 0 && !index)) return eb::rc::BadArgument;
+    GUARD(rt->engine->setPathPerVoice(nodeId, names, numNames, index, voiceBegin, count));
+}
+
 int elem_b200_process(elem_b200_runtime* rt, const float* const* in, size_t nIn, float* const* out, size_t nOut, size_t numSamples, void* userData) {
     GUARD(rt->engine->process(in, nIn, out, nOut, numSamples, static_cast<const int64_t*>(userData)));
 }

@@ -81,6 +81,18 @@ constexpr int TM_THREADS = 2 * TM_GROUP + 32;       // T + M + producer warp
 #endif
 constexpr int TM_STAGES = EB_CONV_TM_STAGES;
 constexpr int TM_CTAS_PER_SM = EB_CONV_TM_CTAS;
+// The per-channel-IR form streams CH input rows and up to CH IR rows per stage (16 KB): 4 stages x 16 KB + 44 KB = 108 KB per CTA,
+// two CTAs per SM still fit in 228 KB (5 stages would not).
+constexpr int PC_STAGES = 4;
+static_assert(CH == 2, "the unit table holds channel pairs");
+
+template <bool PER_CH> struct ConvForm {
+    static constexpr int STAGES = PER_CH ? PC_STAGES : TM_STAGES;
+    static constexpr int HROWS = PER_CH ? CH : 1;     // IR rows per ring stage
+    static constexpr size_t smem() {
+        return (size_t) STAGES * (CH + HROWS) * ROW_BYTES + (size_t) 5 * CH * ROW_BYTES + ROW_BYTES + (2 * STAGES + 8) * sizeof(uint64_t);
+    }
+};
 
 __device__ __forceinline__ void tgroup_sync() { asm volatile("bar.sync 2, %0;" ::"n"(TM_GROUP) : "memory"); }
 
@@ -164,28 +176,60 @@ __device__ __forceinline__ void fft512_t(float2 (*a)[N2], float2 (*b)[N2], const
 #endif
 }
 
+// Relayout of a grown input spectra ring (convolve.h convolver_relayout): one CTA of 128 threads per (channel, new slot).
+__global__ void convolve_ring_relayout_kernel(float2* __restrict__ dst, const float2* __restrict__ src, int oldR, int newR, int cur) {
+    const int ch = blockIdx.x, i = blockIdx.y;
+    float2* d = dst + ((size_t) ch * newR + i) * NB;
+    if (i < oldR) {
+        const int s = (cur + i) % oldR;
+        const float2* p = src + ((size_t) ch * oldR + s) * NB;
+        for (int k = threadIdx.x; k < NB; k += blockDim.x) d[k] = p[k];
+    } else {
+        for (int k = threadIdx.x; k < NB; k += blockDim.x) d[k] = make_float2(0.0f, 0.0f);
+    }
+}
+
 } // namespace
 
+// PER_CH = false: every channel convolves with H (S partitions); units are the channel pairs (2u, 2u + 1).
+// PER_CH = true: channel c convolves with chan[c].H (chan[c].S partitions); unit u is the pair units[u] = {c0, c1 (-1: none), max S,
+// same IR} and its ring stages carry one IR row (same IR) or two.  A channel past its own S contributes nothing (predicated MAC), so
+// a channel's output is bit-identical to the shared form on the same IR.  In both forms the ring has R slots (R >= every S).
+template <bool PER_CH>
 __global__ void __launch_bounds__(TM_THREADS, TM_CTAS_PER_SM) convolve_chunk_tm_kernel(
-    const float* __restrict__ in, int inStride, float* __restrict__ out, int stride, int offset, int n, int fill, int cur, int S, int nv,
-    const float2* __restrict__ H, float2* __restrict__ fdl, float2* __restrict__ ypre,
+    const float* __restrict__ in, int inStride, float* __restrict__ out, int stride, int offset, int n, int fill, int cur, int S, int R, int nv,
+    const float2* __restrict__ H, const ConvChannel* __restrict__ chan, const int4* __restrict__ units,
+    float2* __restrict__ fdl, float2* __restrict__ ypre,
     float* __restrict__ overlap, float* __restrict__ inbuf, const float2* __restrict__ twg, const ConvEpilogue epi) {
+    constexpr int STAGES = ConvForm<PER_CH>::STAGES, HROWS = ConvForm<PER_CH>::HROWS;
     extern __shared__ __align__(128) unsigned char smemRaw[];
-    float2 (*stX)[CH][N2] = reinterpret_cast<float2 (*)[CH][N2]>(smemRaw);                                        // [TM_STAGES][CH][512]
-    float2 (*stH)[N2] = reinterpret_cast<float2 (*)[N2]>(smemRaw + (size_t) TM_STAGES * CH * ROW_BYTES);          // [TM_STAGES][512]
-    float2 (*Xb)[CH][N2] = reinterpret_cast<float2 (*)[CH][N2]>(smemRaw + (size_t) TM_STAGES * (CH + 1) * ROW_BYTES);   // [2][CH][512]
+    float2 (*stX)[CH][N2] = reinterpret_cast<float2 (*)[CH][N2]>(smemRaw);                                        // [STAGES][CH][512]
+    float2 (*stH)[HROWS][N2] = reinterpret_cast<float2 (*)[HROWS][N2]>(smemRaw + (size_t) STAGES * CH * ROW_BYTES);   // [STAGES][HROWS][512]
+    float2 (*Xb)[CH][N2] = reinterpret_cast<float2 (*)[CH][N2]>(smemRaw + (size_t) STAGES * (CH + HROWS) * ROW_BYTES);   // [2][CH][512]
     float2 (*Yb)[CH][N2] = Xb + 2;                                                                                 // [2][CH][512]
     float2 (*Sc)[N2] = reinterpret_cast<float2 (*)[N2]>(Yb + 2);                                                   // [CH][512] transform scratch
     float2* tw = reinterpret_cast<float2*>(Sc + CH);                                                               // [512]
-    uint64_t* full = reinterpret_cast<uint64_t*>(tw + N2);        // [TM_STAGES]
-    uint64_t* empty = full + TM_STAGES;                           // [TM_STAGES]
-    uint64_t* xfull = empty + TM_STAGES;                          // [2] T -> M: Xbuf ready
+    uint64_t* full = reinterpret_cast<uint64_t*>(tw + N2);        // [STAGES]
+    uint64_t* empty = full + STAGES;                              // [STAGES]
+    uint64_t* xfull = empty + STAGES;                             // [2] T -> M: Xbuf ready
     uint64_t* xempty = xfull + 2;                                 // [2] M -> T: Xbuf consumed
     uint64_t* yfull = xempty + 2;                                 // [2] M -> T: Ybuf ready
     uint64_t* yempty = yfull + 2;                                 // [2] T -> M: Ybuf consumed
 
     const int tid = threadIdx.x;
     const int numUnits = (nv + CH - 1) / CH;
+    // channels of unit u: ch[c] is a valid channel to address (a missing second channel aliases the first), ok[c] whether it is real
+    auto unitChannels = [&](int u, int (&ch)[CH], bool (&ok)[CH]) {
+        if (PER_CH) {
+            const int4 ud = units[u];
+            ch[0] = ud.x; ok[0] = true;
+            ch[1] = ud.y >= 0 ? ud.y : ud.x; ok[1] = ud.y >= 0;
+        } else {
+#pragma unroll
+            for (int c = 0; c < CH; ++c) { ch[c] = min(u * CH + c, nv - 1); ok[c] = u * CH + c < nv; }
+        }
+    };
+    auto unitS = [&](int u) { return PER_CH ? units[u].z : S; };
 #ifndef EB_CONV_EARLY_PRODUCER
 #define EB_CONV_EARLY_PRODUCER 1   /* 0 = the producer starts behind the CTA barrier like everyone else */
 #endif
@@ -195,34 +239,58 @@ __global__ void __launch_bounds__(TM_THREADS, TM_CTAS_PER_SM) convolve_chunk_tm_
     const bool producerThread = (tid == 2 * TM_GROUP);
     uint32_t pit = 0;                    // producer: stages issued so far
     int pu = blockIdx.x, pi = 1;         // producer: next (unit, partition) to issue
-    auto produceOne = [&]() {
-        const int stg = pit % TM_STAGES;
-        mbar_wait_b(&empty[stg], ((pit / TM_STAGES) & 1) ^ 1);
-        int slotIdx = cur + pi;
-        if (slotIdx >= S) slotIdx -= S;
-        const int ch0 = pu * CH;
-        mbar_expect_tx(&full[stg], (CH + 1) * ROW_BYTES);
-#pragma unroll
-        for (int c = 0; c < CH; ++c)
-            tma_load_1d(&stX[stg][c][0], fdl + ((size_t) min(ch0 + c, nv - 1) * S + slotIdx) * NB, ROW_BYTES, &full[stg]);
-        tma_load_1d(&stH[stg][0], H + (size_t) pi * NB, ROW_BYTES, &full[stg]);
-        ++pit;
-        if (++pi >= S) { pi = 1; pu += gridDim.x; }
+    int puS = 0;                         // producer: partitions of unit pu
+    auto skipEmpty = [&]() {             // units whose channels have at most one partition stream nothing
+        while (pu < numUnits && (puS = unitS(pu)) <= 1) pu += gridDim.x;
     };
+    auto produceOne = [&]() {
+        const int stg = pit % STAGES;
+        mbar_wait_b(&empty[stg], ((pit / STAGES) & 1) ^ 1);
+        int slotIdx = cur + pi;
+        if (slotIdx >= R) slotIdx -= R;
+        int ch[CH]; bool ok[CH];
+        unitChannels(pu, ch, ok);
+        if (PER_CH) {
+            // one IR row when the unit's channels share the IR, else one per channel; a channel past its own S loads its partner's
+            // row (the partner has > pi partitions, since the unit does) and the MAC ignores it
+            const int nH = units[pu].w ? 1 : CH;
+            mbar_expect_tx(&full[stg], (CH + nH) * ROW_BYTES);
+#pragma unroll
+            for (int c = 0; c < CH; ++c)
+                tma_load_1d(&stX[stg][c][0], fdl + ((size_t) ch[c] * R + slotIdx) * NB, ROW_BYTES, &full[stg]);
+            for (int c = 0; c < nH; ++c) {
+                const ConvChannel d = chan[ch[c]], e = chan[ch[c ^ 1]];
+                const float2* h = (pi < d.S) ? d.H : e.H;
+                tma_load_1d(&stH[stg][c][0], h + (size_t) pi * NB, ROW_BYTES, &full[stg]);
+            }
+        } else {
+            mbar_expect_tx(&full[stg], (CH + 1) * ROW_BYTES);
+#pragma unroll
+            for (int c = 0; c < CH; ++c)
+                tma_load_1d(&stX[stg][c][0], fdl + ((size_t) ch[c] * R + slotIdx) * NB, ROW_BYTES, &full[stg]);
+            tma_load_1d(&stH[stg][0][0], H + (size_t) pi * NB, ROW_BYTES, &full[stg]);
+        }
+        ++pit;
+        if (++pi >= puS) { pi = 1; pu += gridDim.x; skipEmpty(); }
+    };
+    const bool streams = fill == 0 && (PER_CH || S > 1);
     if (EB_CONV_EARLY_PRODUCER ? producerThread : (tid == 0)) {
-        for (int i = 0; i < TM_STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], TM_GROUP / 32); }
+        for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], TM_GROUP / 32); }
         for (int i = 0; i < 2; ++i) { mbar_init(&xfull[i], 1); mbar_init(&xempty[i], TM_GROUP / 32); mbar_init(&yfull[i], TM_GROUP / 32); mbar_init(&yempty[i], 1); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         fence_proxy_async();
-        if (EB_CONV_EARLY_PRODUCER && fill == 0 && S > 1)
-            for (int k = 0; k < TM_STAGES && pu < numUnits; ++k) produceOne();
+        if (EB_CONV_EARLY_PRODUCER && streams) {
+            skipEmpty();
+            for (int k = 0; k < STAGES && pu < numUnits; ++k) produceOne();
+        }
     }
     for (int i = tid; i < N2; i += TM_THREADS) tw[i] = twg[i];
     __syncthreads();
 
     if (tid >= 2 * TM_GROUP) {
         // ---------------- producer warp ----------------
-        if (producerThread && fill == 0 && S > 1) {
+        if (producerThread && streams) {
+            if (!EB_CONV_EARLY_PRODUCER) skipEmpty();
             while (pu < numUnits) produceOne();
         }
         return;
@@ -234,24 +302,37 @@ __global__ void __launch_bounds__(TM_THREADS, TM_CTAS_PER_SM) convolve_chunk_tm_
         uint32_t it = 0;
         int nloc = 0;
         for (int u = blockIdx.x; u < numUnits; u += gridDim.x, ++nloc) {
-            const int ch0 = u * CH, b = nloc & 1;
+            const int b = nloc & 1;
+            int ch[CH]; bool ok[CH];
+            unitChannels(u, ch, ok);
+            int cS[CH];                                                    // partitions of each channel's IR
+            const float2* cH[CH];
+#pragma unroll
+            for (int c = 0; c < CH; ++c) {
+                if (PER_CH) { const ConvChannel d = chan[ch[c]]; cS[c] = ok[c] ? d.S : 0; cH[c] = d.H; }
+                else { cS[c] = S; cH[c] = H; }
+            }
+            const int uS = unitS(u);
+            const bool sameIr = !PER_CH || units[u].w != 0;
             float2 acc[4][CH];
             if (fill == 0) {
 #pragma unroll
                 for (int q = 0; q < 4; ++q)
 #pragma unroll
                     for (int c = 0; c < CH; ++c) acc[q][c] = make_float2(0.0f, 0.0f);
-                for (int i = 1; i < S; ++i, ++it) {
-                    const int stg = it % TM_STAGES;
-                    mbar_wait_b(&full[stg], (it / TM_STAGES) & 1);
+                for (int i = 1; i < uS; ++i, ++it) {
+                    const int stg = it % STAGES;
+                    mbar_wait_b(&full[stg], (it / STAGES) & 1);
 #pragma unroll
                     for (int q = 0; q < 4; ++q) {
                         const int k = t + q * TM_GROUP;
-                        const float2 hq = stH[stg][k];
+                        const float2 h0q = stH[stg][0][k];
 #pragma unroll
                         for (int c = 0; c < CH; ++c) {
+                            const float2 hq = (PER_CH && c > 0 && !sameIr) ? stH[stg][HROWS - 1][k] : h0q;
                             const float2 x = stX[stg][c][k];
-                            acc[q][c] = (k == 0) ? make_float2(acc[q][c].x + hq.x * x.x, acc[q][c].y + hq.y * x.y) : cadd(acc[q][c], cmul(hq, x));
+                            if (!PER_CH || i < cS[c])
+                                acc[q][c] = (k == 0) ? make_float2(acc[q][c].x + hq.x * x.x, acc[q][c].y + hq.y * x.y) : cadd(acc[q][c], cmul(hq, x));
                         }
                     }
                     __syncwarp();
@@ -260,21 +341,30 @@ __global__ void __launch_bounds__(TM_THREADS, TM_CTAS_PER_SM) convolve_chunk_tm_
 #pragma unroll
                 for (int q = 0; q < 4; ++q)
 #pragma unroll
-                    for (int c = 0; c < CH; ++c) if (ch0 + c < nv) ypre[(size_t) (ch0 + c) * NB + t + q * TM_GROUP] = acc[q][c];
+                    for (int c = 0; c < CH; ++c) if (ok[c]) ypre[(size_t) ch[c] * NB + t + q * TM_GROUP] = acc[q][c];
             } else {
 #pragma unroll
                 for (int q = 0; q < 4; ++q)
 #pragma unroll
-                    for (int c = 0; c < CH; ++c) acc[q][c] = ypre[(size_t) min(ch0 + c, nv - 1) * NB + t + q * TM_GROUP];
+                    for (int c = 0; c < CH; ++c) acc[q][c] = ypre[(size_t) ch[c] * NB + t + q * TM_GROUP];
             }
             mbar_wait_b(&xfull[b], (nloc >> 1) & 1);                       // the forward transform of this pair is in Xbuf[b]
             mbar_wait_b(&yempty[b], ((nloc >> 1) & 1) ^ 1);                // the inverse transform of pair n-2 has left Ybuf[b]
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
                 const int k = t + q * TM_GROUP;
-                const float2 h0 = __ldg(H + k);
+                // the newest partition against each channel's own H_0 (an IR trimmed to nothing: zero)
+                float2 h0s[CH];
 #pragma unroll
                 for (int c = 0; c < CH; ++c) {
+                    if (!PER_CH) h0s[c] = (c == 0) ? __ldg(H + k) : h0s[0];
+                    else if (cS[c] == 0) h0s[c] = make_float2(0.0f, 0.0f);
+                    else if (c > 0 && sameIr) h0s[c] = h0s[0];
+                    else h0s[c] = __ldg(cH[c] + k);
+                }
+#pragma unroll
+                for (int c = 0; c < CH; ++c) {
+                    const float2 h0 = h0s[c];
                     const float2 x = Xb[b][c][k];
                     Yb[b][c][k] = (k == 0) ? make_float2(acc[q][c].x + x.x * h0.x, acc[q][c].y + x.y * h0.y) : cadd(acc[q][c], cmul(x, h0));
                 }
@@ -291,18 +381,20 @@ __global__ void __launch_bounds__(TM_THREADS, TM_CTAS_PER_SM) convolve_chunk_tm_
     const float scale = 1.0f / 512.0f;
 
     auto forward = [&](int u, int nloc) {
-        const int ch0 = u * CH, b = nloc & 1;
+        const int b = nloc & 1;
+        int chs[CH]; bool oks[CH];
+        unitChannels(u, chs, oks);
         if (t == 0) mbar_wait_b(&xempty[b], ((nloc >> 1) & 1) ^ 1);       // M is done with what Xbuf[b] held (pair n-2)
         tgroup_sync();
         if (wholeBlock) {
 #pragma unroll
             for (int c = 0; c < CH; ++c) {
-                const int ch = ch0 + c;
+                const int ch = chs[c];
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                     const int k = t + h * TM_GROUP;
                     float2 z = make_float2(0.0f, 0.0f);
-                    if (ch < nv) z = __ldg(reinterpret_cast<const float2*>(in + (size_t) ch * inStride + offset) + k);
+                    if (oks[c]) z = __ldg(reinterpret_cast<const float2*>(in + (size_t) ch * inStride + offset) + k);
                     Sc[c][k] = z;
                     Sc[c][k + 256] = make_float2(0.0f, 0.0f);
                 }
@@ -310,8 +402,8 @@ __global__ void __launch_bounds__(TM_THREADS, TM_CTAS_PER_SM) convolve_chunk_tm_
         } else {
 #pragma unroll
             for (int c = 0; c < CH; ++c) {
-                const int ch = ch0 + c;
-                if (ch < nv) {
+                const int ch = chs[c];
+                if (oks[c]) {
                     float* ib = inbuf + (size_t) ch * CONV_BLOCK;
                     for (int i = t; i < n; i += TM_GROUP) ib[fill + i] = in[(size_t) ch * inStride + offset + i];
                 }
@@ -319,12 +411,12 @@ __global__ void __launch_bounds__(TM_THREADS, TM_CTAS_PER_SM) convolve_chunk_tm_
             tgroup_sync();
 #pragma unroll
             for (int c = 0; c < CH; ++c) {
-                const int ch = ch0 + c;
+                const int ch = chs[c];
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                     const int k = t + h * TM_GROUP;
                     float2 z = make_float2(0.0f, 0.0f);
-                    if (ch < nv) z = reinterpret_cast<const float2*>(inbuf + (size_t) ch * CONV_BLOCK)[k];
+                    if (oks[c]) z = reinterpret_cast<const float2*>(inbuf + (size_t) ch * CONV_BLOCK)[k];
                     Sc[c][k] = z;
                     Sc[c][k + 256] = make_float2(0.0f, 0.0f);
                 }
@@ -335,8 +427,8 @@ __global__ void __launch_bounds__(TM_THREADS, TM_CTAS_PER_SM) convolve_chunk_tm_
         // split in place: bins k and 512-k are produced together from Z[k], Z[512-k]; bin 512 is packed into bin 0
 #pragma unroll
         for (int c = 0; c < CH; ++c) {
-            const int ch = ch0 + c;
-            float2* slot = fdl + ((size_t) min(ch, nv - 1) * S + cur) * NB;
+            const bool ok = oks[c];
+            float2* slot = fdl + ((size_t) chs[c] * R + cur) * NB;
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int k = t + h * TM_GROUP;                            // 0..255
@@ -348,7 +440,7 @@ __global__ void __launch_bounds__(TM_THREADS, TM_CTAS_PER_SM) convolve_chunk_tm_
                     const float2 oh = make_float2(0.5f * dh.y, -0.5f * dh.x);
                     const float2 xh = cadd(eh, cmul(tw[256], oh));
                     Xb[b][c][0] = x0; Xb[b][c][256] = xh;
-                    if (ch < nv) { slot[0] = x0; slot[256] = xh; }
+                    if (ok) { slot[0] = x0; slot[256] = xh; }
                 } else {
                     const int kn = N2 - k;
                     const float2 zk = Xb[b][c][k], zq = Xb[b][c][kn];
@@ -364,7 +456,7 @@ __global__ void __launch_bounds__(TM_THREADS, TM_CTAS_PER_SM) convolve_chunk_tm_
                     const float2 o2 = make_float2(0.5f * d2.y, -0.5f * d2.x);
                     const float2 xn = cadd(e2, cmul(tw[kn], o2));
                     Xb[b][c][k] = xk; Xb[b][c][kn] = xn;
-                    if (ch < nv) { slot[k] = xk; slot[kn] = xn; }
+                    if (ok) { slot[k] = xk; slot[kn] = xn; }
                 }
             }
         }
@@ -373,12 +465,14 @@ __global__ void __launch_bounds__(TM_THREADS, TM_CTAS_PER_SM) convolve_chunk_tm_
     };
 
     auto inverse = [&](int u, int nloc) {
-        const int ch0 = u * CH, b = nloc & 1;
+        const int b = nloc & 1;
+        int chs[CH]; bool oks[CH];
+        unitChannels(u, chs, oks);
         // overlap of the previous partition for this chunk: fetched before waiting, used after the inverse FFT
         float ovv[CH][4];
 #pragma unroll
         for (int c = 0; c < CH; ++c) {
-            const float* ov = overlap + (size_t) min(ch0 + c, nv - 1) * CONV_BLOCK;
+            const float* ov = overlap + (size_t) chs[c] * CONV_BLOCK;
 #pragma unroll
             for (int q = 0; q < 4; ++q) { const int i = t + q * TM_GROUP; ovv[c][q] = (i < n) ? ov[fill + i] : 0.0f; }
         }
@@ -419,8 +513,8 @@ __global__ void __launch_bounds__(TM_THREADS, TM_CTAS_PER_SM) convolve_chunk_tm_
         if (t == 0) mbar_arrive(&yempty[b]);                                // Ybuf[b] may be overwritten (pair n+2)
 #pragma unroll
         for (int c = 0; c < CH; ++c) {
-            const int ch = ch0 + c;
-            if (ch >= nv) continue;
+            const int ch = chs[c];
+            if (!oks[c]) continue;
             const float* y = reinterpret_cast<const float*>(&Sc[c][0]);
             if (!epi.active) {
                 float* o = out + (size_t) ch * stride + offset;
@@ -453,8 +547,8 @@ __global__ void __launch_bounds__(TM_THREADS, TM_CTAS_PER_SM) convolve_chunk_tm_
         if (fill + n == CONV_BLOCK) {
 #pragma unroll
             for (int c = 0; c < CH; ++c) {
-                const int ch = ch0 + c;
-                if (ch >= nv) continue;
+                const int ch = chs[c];
+                if (!oks[c]) continue;
                 const float* y = reinterpret_cast<const float*>(&Sc[c][0]);
                 float* ov = overlap + (size_t) ch * CONV_BLOCK;
                 float* ib = inbuf + (size_t) ch * CONV_BLOCK;
@@ -476,7 +570,7 @@ __global__ void __launch_bounds__(TM_THREADS, TM_CTAS_PER_SM) convolve_chunk_tm_
 cudaError_t convolver_process_chunk(ConvolverState& st, const float* in, int inStride, float* out, int stride, int offset, int n, cudaStream_t stream,
                                     const ConvEpilogue& epi) {
     if (st.planOnly) return cudaErrorNotSupported;
-    if (st.partitions == 0) {   // empty (fully trimmed) IR: silence (FFTConvolver.cpp:149-153)
+    if (st.maxS == 0) {   // empty (fully trimmed) IR on every channel: silence (FFTConvolver.cpp:149-153)
         if (epi.active) {
             cudaError_t e = cudaSuccess;
             if (epi.mixPartial) e = cudaMemset2DAsync(epi.mixPartial + (size_t) epi.tileBase * epi.nOut * epi.blockSize + offset, sizeof(float) * epi.blockSize, 0, sizeof(float) * n, (size_t) st.nv * epi.nOut, stream);
@@ -487,9 +581,11 @@ cudaError_t convolver_process_chunk(ConvolverState& st, const float* in, int inS
     }
     const int units = (st.nv + CONV_CH_PER_CTA - 1) / CONV_CH_PER_CTA;
     static int smCount = 0;
-    const size_t smem = (size_t) TM_STAGES * (CH + 1) * ROW_BYTES + (size_t) 5 * CH * ROW_BYTES + ROW_BYTES + (2 * TM_STAGES + 8) * sizeof(uint64_t);
+    const bool perCh = st.perChannel();
+    const size_t smem = perCh ? ConvForm<true>::smem() : ConvForm<false>::smem();
     if (smCount == 0) {
-        cudaError_t e = cudaFuncSetAttribute(convolve_chunk_tm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
+        cudaError_t e = cudaFuncSetAttribute(convolve_chunk_tm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ConvForm<false>::smem());
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(convolve_chunk_tm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) ConvForm<true>::smem());
         if (e != cudaSuccess) return e;
         int dev = 0;
         cudaGetDevice(&dev);
@@ -507,13 +603,23 @@ cudaError_t convolver_process_chunk(ConvolverState& st, const float* in, int inS
         const int rounds = (units + persistent - 1) / persistent;
         grid = (units + rounds - 1) / rounds;
     }
-    convolve_chunk_tm_kernel<<<grid, TM_THREADS, smem, stream>>>(in, inStride, out, stride, offset, n, st.fill, st.cur, st.partitions, st.nv,
-                                                                st.dH, st.dFdl, st.dYpre, st.dOverlap, st.dInBuf, st.dTw, epi);
+    if (perCh)
+        convolve_chunk_tm_kernel<true><<<grid, TM_THREADS, smem, stream>>>(in, inStride, out, stride, offset, n, st.fill, st.cur, 0, st.partitions, st.nv,
+                                                                          nullptr, st.dChan, st.dUnits, st.dFdl, st.dYpre, st.dOverlap, st.dInBuf, st.dTw, epi);
+    else   // one IR for every channel (its S may be below the ring's R after reassignments)
+        convolve_chunk_tm_kernel<false><<<grid, TM_THREADS, smem, stream>>>(in, inStride, out, stride, offset, n, st.fill, st.cur, st.maxS, st.partitions, st.nv,
+                                                                           st.irs[0]->dH, nullptr, nullptr, st.dFdl, st.dYpre, st.dOverlap, st.dInBuf, st.dTw, epi);
     st.fill += n;
     if (st.fill == CONV_BLOCK) {
         st.fill = 0;
         st.cur = (st.cur > 0) ? st.cur - 1 : st.partitions - 1;   // FFTConvolver.cpp:200
     }
+    return cudaGetLastError();
+}
+
+cudaError_t convolver_relayout(float2* dst, const float2* src, int nv, int oldR, int newR, int cur, cudaStream_t stream) {
+    if (nv == 0 || newR == 0) return cudaSuccess;
+    convolve_ring_relayout_kernel<<<dim3(nv, newR), 128, 0, stream>>>(dst, src, oldR, newR, cur);
     return cudaGetLastError();
 }
 

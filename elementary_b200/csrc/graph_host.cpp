@@ -276,9 +276,23 @@ std::string Engine::describe() const {
                 }
             }
         }
+        // K3 state per convolver: distinct IRs in use and the kernel form that runs (silent: every IR trimmed to nothing)
+        std::map<int32_t, const ConvolverState*> convs;
+        for (auto& kv : g->nodes) if (kv.second.kind == NodeKind::Convolve && kv.second.conv) convs[kv.first] = kv.second.conv.get();
+        if (!convs.empty()) {
+            os << ",\"convolvers\":[";
+            bool firstConv = true;
+            for (auto& kv : convs) {
+                const ConvolverState& cs = *kv.second;
+                os << (firstConv ? "" : ",") << "{\"node\":" << kv.first << ",\"irs\":" << cs.irs.size() << ",\"partitions\":" << cs.partitions
+                   << ",\"form\":\"" << (cs.maxS == 0 ? "silent" : (cs.perChannel() ? "per_channel" : "shared")) << "\"}";
+                firstConv = false;
+            }
+            os << "]";
+        }
         os << "}";
     }
-    os << "]}";
+    os << "],\"ir_bank\":" << irBank_.live() << "}";
     return os.str();
 }
 
@@ -934,7 +948,8 @@ int Engine::splitGroupsAt(int v) {
                 std::string err;
                 if (!convolver_clone_range(*kv.second.conv, cut, ng->nv, *cs, stream_, err)) return fail(rc::CudaError, err);
                 n.conv = cs;
-                kv.second.conv->nv = cut;   // the old state keeps its (now partly unused) storage
+                // the old state keeps its (now partly unused) storage
+                if (!convolver_truncate(*kv.second.conv, cut, stream_, err)) return fail(rc::CudaError, err);
             }
             ng->nodes.emplace(kv.first, std::move(n));
         }
@@ -1091,6 +1106,66 @@ int Engine::setPropertyPerVoice(int32_t nodeId, const char* key, const double* v
         } else return fail(rc::InvalidPropertyType, "property is not per-voice capable");
         if (!cuda(dmemcpy(g.dRows + (size_t) row * g.Vpad + (b - g.v0), bits.data(), sizeof(uint32_t) * bits.size(), cudaMemcpyHostToDevice), "per-voice prop upload")) return rc::CudaError;   // pageable source: staged before the call returns
         n.props[k] = Value::number(values[e - 1 - vb]);
+    }
+    return rc::Ok;
+}
+
+int Engine::setPathPerVoice(int32_t nodeId, const char* const* names, int numNames, const int32_t* index, int vb, int count) {
+    Lock lk(mu_);
+    dsetdev();
+    if (vb < 0 || count < 0 || vb + count > numVoices_ || numNames < 0) return fail(rc::BadArgument, "voice range out of bounds");
+    for (int i = 0; i < count; ++i)
+        if (index[i] < 0 || index[i] >= numNames) return fail(rc::BadArgument, "name index out of range");
+    // every check before any change: a failed call changes nothing
+    for (auto& gp : groups_) {
+        const Group& g = *gp;
+        if (std::max(vb, g.v0) >= std::min(vb + count, g.v0 + g.nv)) continue;
+        auto it = g.nodes.find(nodeId);
+        if (it == g.nodes.end()) return rc::NodeNotFound;
+        if (it->second.kind != NodeKind::Convolve) return fail(rc::InvalidPropertyType, "property is not per-voice capable");
+    }
+    std::vector<std::shared_ptr<Resource>> res((size_t) numNames);
+    for (int k = 0; k < numNames; ++k) {
+        auto it = names[k] ? resources_.find(names[k]) : resources_.end();
+        if (it == resources_.end()) return fail(rc::InvalidPropertyValue, std::string("no shared resource named ") + (names[k] ? names[k] : "(null)"));
+        res[(size_t) k] = it->second;
+    }
+    if (count == 0) return rc::Ok;
+    steadyValid_ = false;
+    std::vector<std::shared_ptr<IrSpectra>> spectra((size_t) numNames);   // computed (or found in the bank) once per name
+    auto spectraOf = [&](int k, std::string& err) -> std::shared_ptr<IrSpectra> {
+        if (!spectra[(size_t) k]) {
+            const Resource& r = *res[(size_t) k];
+            static const std::vector<float> none;
+            const auto& ch0 = r.channels.empty() ? none : r.channels[0];
+            spectra[(size_t) k] = irBank_.acquire(&r, res[(size_t) k], ch0.data(), ch0.size(), planOnly_, stream_, err);
+        }
+        return spectra[(size_t) k];
+    };
+    for (auto& gp : groups_) {
+        Group& g = *gp;
+        const int b = std::max(vb, g.v0), e = std::min(vb + count, g.v0 + g.nv);
+        if (b >= e) continue;
+        Node& n = g.nodes.find(nodeId)->second;
+        std::string err;
+        const bool hadResource = (bool) n.resource;
+        if (n.resourceDirty || !n.conv) {
+            // the whole-group state the next compile would have made (a fresh convolver on the node's `path`, or none: silence)
+            auto cs = std::make_shared<ConvolverState>();
+            static const std::vector<float> none;
+            const auto& ch0 = (!n.resource || n.resource->channels.empty()) ? none : n.resource->channels[0];
+            if (!convolver_init(*cs, irBank_, n.resource.get(), n.resource, ch0.data(), ch0.size(), g.nv, planOnly_, stream_, err)) return fail(rc::CudaError, err);
+            n.conv = cs;
+            n.resourceDirty = false;
+        }
+        std::vector<std::shared_ptr<IrSpectra>> h((size_t) (e - b));
+        for (int v = b; v < e; ++v)
+            if (!(h[(size_t) (v - b)] = spectraOf(index[v - vb], err))) return fail(rc::CudaError, err);
+        if (!convolver_assign(*n.conv, b - g.v0, e - b, h, stream_, err)) return fail(rc::CudaError, err);
+        const int last = index[e - 1 - vb];   // snapshot(): the value last set for the group's highest addressed voice
+        n.resource = res[(size_t) last];
+        n.props["path"] = Value::string(names[last]);
+        if (!hadResource) g.codeDirty = true;   // the program emitted silence for a convolver without an IR
     }
     return rc::Ok;
 }
@@ -1427,7 +1502,7 @@ int Compiler::emitNode(Node& n, int rootIndex) {
                 auto cs = std::make_shared<ConvolverState>();
                 const auto& ch0 = n.resource->channels.empty() ? std::vector<float>() : n.resource->channels[0];
                 std::string err;
-                if (!convolver_init(*cs, ch0.data(), ch0.size(), g.nv, E.planOnly_, E.stream_, err)) return E.fail(rc::CudaError, err);
+                if (!convolver_init(*cs, E.irBank_, n.resource.get(), n.resource, ch0.data(), ch0.size(), g.nv, E.planOnly_, E.stream_, err)) return E.fail(rc::CudaError, err);
                 n.conv = cs;
                 n.resourceDirty = false;
             }
@@ -2423,7 +2498,7 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
                 }
                 int offset = 0;
                 while (offset < (int) numSamples) {
-                    const int n = cs.partitions == 0 ? (int) numSamples - offset
+                    const int n = cs.maxS == 0 ? (int) numSamples - offset
                                                      : std::min((int) numSamples - offset, CONV_BLOCK - cs.fill);
                     std::pair<cudaEvent_t, cudaEvent_t> ev3{nullptr, nullptr};
                     if (timeKernels_) {

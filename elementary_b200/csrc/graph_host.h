@@ -13,6 +13,7 @@
 #include <unordered_map>
 #include <vector>
 
+#include "convolve.h"
 #include "kernels.h"
 #include "program.h"
 #include "value.h"
@@ -197,6 +198,10 @@ public:
     // count): nProps copies straight from the caller's table, no per-value conversion, no JSON.
     int applyBinary(int voiceBegin, int voiceEnd, const void* data, size_t bytes);
     int setConstTable(const int32_t* nodeIds, int nProps, const float* values, int voiceBegin, int count);
+    // Per-voice `path` of a convolve node: voice voiceBegin+i convolves with the shared resource names[index[i]] from the next block
+    // on, restarting from silence like a [3, nodeId, "path", name] batch on that voice alone — but the voice group is not cut: the
+    // group's K3 state holds one IR per channel (convolve.h).  Everything is checked before anything changes.
+    int setPathPerVoice(int32_t nodeId, const char* const* names, int numNames, const int32_t* index, int voiceBegin, int count);
     int addSharedResource(const char* name, const float* const* chans, size_t nCh, size_t nSamples);
     void pruneSharedResources();
     std::vector<std::string> listSharedResources() const;
@@ -283,6 +288,7 @@ private:
     EngineOptions opt_;
     std::vector<std::unique_ptr<Group>> groups_;
     std::map<std::string, std::shared_ptr<Resource>> resources_;
+    IrBank irBank_;                       // convolver IR spectra, one set per resource however many channels use it
     struct CustomType { std::string name, body; int nIn = 0, nState = 0; };
     std::vector<CustomType> customTypes_;
     std::string customSource() const;     // the generated device text of all registered types (part of the specialisation key)

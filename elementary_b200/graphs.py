@@ -85,15 +85,26 @@ def convolve_channel(path: str = "ir") -> List[list]:
     return el.render(el.convolve({"path": path}, el.in_(0)))
 
 
-def lcg_ir(taps: int = 16384) -> "list[float]":
-    """16384-tap decaying-noise IR: s = s*1664525 + 1013904223 (s0 = 1), x = ((s>>8)/2^24 - 0.5)*0.01*exp(-6 n/N)."""
-    s = 1
-    out = []
-    for n in range(taps):
-        s = (s * 1664525 + 1013904223) & 0xFFFFFFFF
-        x = ((s >> 8) / float(1 << 24) - 0.5) * 0.01
-        out.append(x * math.exp(-6.0 * n / taps))
-    return out
+def lcg_ir(taps: int = 16384, seed: int = 1) -> "list[float]":
+    """16384-tap decaying-noise IR: s = s*1664525 + 1013904223 (s0 = seed), x = ((s>>8)/2^24 - 0.5)*0.01*exp(-6 n/N).
+
+    The generator states come from a prefix scan of the affine maps s -> a*s + c (log2(taps) numpy steps, arithmetic mod 2^64,
+    which is exact mod 2^32), so a thousand IRs take milliseconds each; the values are those of the plain sequential loop."""
+    import numpy as np
+    if taps <= 0:
+        return []
+    mask = np.uint64(0xFFFFFFFF)
+    A = np.full(taps, 1664525, dtype=np.uint64)          # after round k, entry i maps s0 to s_{min(i+1, 2k)}
+    C = np.full(taps, 1013904223, dtype=np.uint64)
+    k = 1
+    while k < taps:
+        ak, ck = A[k - 1], C[k - 1]
+        A[k:], C[k:] = (A[:-k] * ak) & mask, (C[:-k] * ak + ck) & mask
+        k *= 2
+    s = (A * np.uint64(seed & 0xFFFFFFFF) + C) & mask
+    x = ((s >> np.uint64(8)).astype(np.float64) / float(1 << 24) - 0.5) * 0.01
+    env = np.array([math.exp(-6.0 * n / taps) for n in range(taps)])   # math.exp: the same bits as the loop it replaces
+    return (x * env).tolist()
 
 
 # --- config 5: random 64-node graphs ----------------------------------------------------------------------------

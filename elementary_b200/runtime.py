@@ -60,6 +60,8 @@ def load_library() -> C.CDLL:
     lib.elem_b200_set_const_table.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int, _f32p, C.c_int, C.c_int]
     lib.elem_b200_set_property_per_voice.restype = C.c_int
     lib.elem_b200_set_property_per_voice.argtypes = [C.c_void_p, C.c_int32, C.c_char_p, C.POINTER(C.c_double), C.c_int, C.c_int]
+    lib.elem_b200_set_path_per_voice.restype = C.c_int
+    lib.elem_b200_set_path_per_voice.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), C.c_int, C.POINTER(C.c_int32), C.c_int, C.c_int]
     lib.elem_b200_process.restype = C.c_int
     lib.elem_b200_process.argtypes = [C.c_void_p, _f32pp, C.c_size_t, _f32pp, C.c_size_t, C.c_size_t, C.c_void_p]
     lib.elem_b200_set_current_time.argtypes = [C.c_void_p, C.c_int64]
@@ -202,6 +204,15 @@ class Runtime:
         v = np.ascontiguousarray(np.asarray(values, dtype=np.float64))
         return self._lib.elem_b200_set_property_per_voice(self._h, int(node_id), key.encode(),
                                                           v.ctypes.data_as(C.POINTER(C.c_double)), int(voice_begin), v.size)
+
+    def set_path_per_voice(self, node_id: int, names, index, voice_begin: int = 0) -> int:
+        """Voice ``voice_begin + i`` of convolve node ``node_id`` gets the impulse response ``names[index[i]]`` (shared resources),
+        without cutting its voice group; the addressed voices restart from silence at the next block."""
+        enc = [n.encode() if isinstance(n, str) else bytes(n) for n in names]
+        tab = (C.c_char_p * max(1, len(enc)))(*enc)
+        idx = np.ascontiguousarray(np.asarray(index, dtype=np.int32).reshape(-1))
+        return self._lib.elem_b200_set_path_per_voice(self._h, int(node_id), tab, len(enc),
+                                                      idx.ctypes.data_as(C.POINTER(C.c_int32)), int(voice_begin), idx.size)
 
     # -- Runtime::process (Runtime.h:51-57,275-290): out = mix bus over all voices -------------------------------
     def process(self, inputs: Optional[np.ndarray], num_outputs: int, num_samples: Optional[int] = None,

@@ -64,6 +64,18 @@ int elem_b200_set_const_table(elem_b200_runtime* rt, const int32_t* nodeIds, int
 int elem_b200_set_property_per_voice(elem_b200_runtime* rt, int32_t nodeId, const char* key,
                                      const double* values, int voiceBegin, int count);
 
+/* Per-voice impulse response of a `convolve` node (ConvolutionNode::setProperty("path"), wasm/Convolve.h:34-56).
+ * voice voiceBegin+i gets the `path` names[index[i]]; same result as `count` single-voice
+ * [[3, nodeId, "path", names[index[i]]]] batches, except that no voice group is cut.
+ * A names table plus a per-voice index, like elem_b200_set_const_table: a million voices choose among K IRs without a million strings.
+ * Each addressed voice restarts from silence (a fresh convolver, even on an unchanged name) at the next process/enqueue_block;
+ * the other voices are untouched.  Each resource's partition spectra are computed once, however many voices use it.
+ * Returns -2 for a voice range out of bounds or an index outside [0, numNames), NodeNotFound (2) when a voice group in the range
+ * lacks the node, InvalidPropertyType (5) when the node is not a convolve, InvalidPropertyValue (6) when a name is not a shared
+ * resource.  All of it is checked before anything changes: a failed call changes nothing. */
+int elem_b200_set_path_per_voice(elem_b200_runtime* rt, int32_t nodeId, const char* const* names, int numNames,
+                                 const int32_t* index, int voiceBegin, int count);
+
 /* Runtime::process(in, nIn, out, nOut, numSamples, userData) — Runtime.h:51-57,275-290.
  * `in` channels are broadcast to every voice; out[c] receives the MIX BUS: the sum over all voices of what
  * each voice's Runtime would have written to its out[c].  Host buffers; the H2D copy of the inputs and the hand-over of the
