@@ -40,7 +40,7 @@ namespace {
 
 constexpr float kEps = FLT_EPSILON;
 #ifndef EB_SVF_SCAN_MAX_L
-#define EB_SVF_SCAN_MAX_L 4      // tiles of up to this many voices run the svf tick as a warp scan (render_ops.inc, OP_SVF)
+#define EB_SVF_SCAN_MAX_L 4      // tiles of up to this many voices run the svf tick as a register-blocked warp scan (render_ops.inc, OP_SVF)
 #endif
 constexpr unsigned FULL = 0xFFFFFFFFu;
 
@@ -181,6 +181,19 @@ __device__ __forceinline__ double tan_quarter_wave(double x) {
     c = fma(c, y2, -0.5);
     c = fma(c, y2, 1.0);
     return big ? div_fast(c, s) : div_fast(s, c);
+}
+
+// The svf tick is an affine map of its double state, s' = M s + c (render_ops.inc, OP_SVF).  affine_then(a, b) is map a applied
+// after map b: M = M_a M_b, c = M_a c_b + c_a — the one composition rule of the per-lane fold and of the warp scan.
+struct Affine2 { double m00, m01, m10, m11, c0, c1; };
+__device__ __forceinline__ Affine2 affine_then(const Affine2& a, const Affine2& b) {
+    return {fma(a.m00, b.m00, a.m01 * b.m10), fma(a.m00, b.m01, a.m01 * b.m11),
+            fma(a.m10, b.m00, a.m11 * b.m10), fma(a.m10, b.m01, a.m11 * b.m11),
+            fma(a.m00, b.c0, fma(a.m01, b.c1, a.c0)), fma(a.m10, b.c0, fma(a.m11, b.c1, a.c1))};
+}
+__device__ __forceinline__ Affine2 affine_shfl_up(const Affine2& a, int delta) {
+    return {__shfl_up_sync(FULL, a.m00, delta), __shfl_up_sync(FULL, a.m01, delta), __shfl_up_sync(FULL, a.m10, delta),
+            __shfl_up_sync(FULL, a.m11, delta), __shfl_up_sync(FULL, a.c0, delta), __shfl_up_sync(FULL, a.c1, delta)};
 }
 
 // svf coefficients of one sample (SVF.h:72-80) out of line, for the 128-sample one-voice tiles (see sin_f32_ool): g, a1 = 1/(1 + g (g + k))
