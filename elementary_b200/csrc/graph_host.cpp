@@ -2561,7 +2561,7 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
         }
         int wpc = opt_.warpsPerCta;
         if (wpc <= 0) wpc = total >= smCount_ * 8 ? 4 : (total >= smCount_ * 4 ? 2 : 1);
-        while (wpc > 1 && render_smem_bytes(maxSlots, (int) nOut, maxState, maxParams, wpc, L, L == 1 ? opt_.niter : 0) > 200 * 1024) wpc >>= 1;
+        while (wpc > 1 && render_smem_bytes(maxSlots, (int) nOut, maxState, maxParams, wpc, L, opt_.niter) > 200 * 1024) wpc >>= 1;
         std::pair<cudaEvent_t, cudaEvent_t> ev{nullptr, nullptr};
         if (timeKernels_) {
             if (!eventPool_.empty()) { ev = eventPool_.back(); eventPool_.pop_back(); }

@@ -1079,10 +1079,15 @@ cudaError_t launch_render_groups(const LaunchParams* descs, const int* tileStart
     if (totalTiles <= 0) return cudaSuccess;
     const int grid = (totalTiles + warpsPerCta - 1) / warpsPerCta;
     const int threads = warpsPerCta * 32;
-    if (tileWidth != 1) niterOverride = 0;       // the many-groups launch has the T = 128 variant for one-voice tiles only
+    // the same sample-tile length as the single-group launch of the geometry (render_niter_for): a group that is cut keeps its
+    // tile length, so its samples stay the same bits (the svf scan, for one, depends on it)
     const size_t smem = render_smem_bytes(maxSlots, nOut, maxStateRows, maxParams, warpsPerCta, tileWidth, niterOverride);
     if (tileWidth == 1 && render_niter_for(1, niterOverride) == 4)
         return launch_groups_impl<4, 0>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, stream);
+    if (tileWidth == 2 && render_niter_for(2, niterOverride) == 8)
+        return launch_groups_impl<8, 1>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, stream);
+    if (tileWidth == 32 && render_niter_for(32, niterOverride) == 4)
+        return launch_groups_impl<4, 5>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, stream);
     switch (tileWidth) {
         case 32: return launch_groups_impl<8, 5>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, stream);
         case 16: return launch_groups_impl<8, 4>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, stream);
