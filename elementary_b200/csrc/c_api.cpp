@@ -10,6 +10,8 @@
 #include "graph_host.h"
 #include "kernels.h"
 
+static_assert(eb::MAX_WIDE_OUT_CHANNELS == ELEM_B200_MAX_OUT_CHANNELS, "the header documents the output channel cap");
+
 struct elem_b200_runtime {
     eb::Engine* engine;
     std::string scratch;

@@ -160,6 +160,7 @@ Engine::Engine(double sampleRate, int blockSize, int numVoices, int device)
     auto g = std::make_unique<Group>();
     g->v0 = 0; g->nv = numVoices_; g->Vpad = (numVoices_ + 31) / 32 * 32;
     groups_.push_back(std::move(g));
+    mixFloats_ = (size_t) MAX_OUT_CHANNELS * blockSize_;
     cuda(dmalloc((void**) &dMix_, sizeof(float) * MAX_OUT_CHANNELS * blockSize_), "cudaMalloc mix");
     if (dMix_) cuda(dmemset(dMix_, 0, sizeof(float) * MAX_OUT_CHANNELS * blockSize_), "memset mix");
     if (!planOnly_) {
@@ -211,6 +212,12 @@ Engine::~Engine() {
     if (hMixHost_) cudaFreeHost(hMixHost_);
     for (int i = 0; i < 2; ++i) { if (offlineDev_[i]) cudaFree(offlineDev_[i]); if (offlinePinned_[i]) cudaFreeHost(offlinePinned_[i]); }
     if (dDeliverDone_) cudaFree(dDeliverDone_);
+    if (wide_.dRows) dfree(wide_.dRows);
+    if (wide_.dSegs) dfree(wide_.dSegs);
+    if (wide_.dDst) dfree(wide_.dDst);
+    if (dWideScratch_) dfree(dWideScratch_);
+    if (dWideTickets_) dfree(dWideTickets_);
+    if (dOutCompact_) dfree(dOutCompact_);
     for (auto& kv : batch_) { if (kv.second.dDescs) dfree(kv.second.dDescs); if (kv.second.dTileStart) dfree(kv.second.dTileStart); }
     for (auto* l : {&timedEvents_, &timedMixEvents_, &timedConvEvents_, &timedXchgEvents_})
         for (auto& ev : *l) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
@@ -251,7 +258,7 @@ int Engine::setOption(const char* key, double value) {
 std::string Engine::describe() const {
     Lock lk(mu_);
     std::ostringstream os;
-    os << "{\"voices\":" << numVoices_ << ",\"groups\":[";
+    os << "{\"voices\":" << numVoices_ << ",\"steady\":" << (steadyValid_ ? "true" : "false") << ",\"groups\":[";
     bool first = true;
     for (auto& g : groups_) {
         if (!first) os << ",";
@@ -261,6 +268,12 @@ std::string Engine::describe() const {
             auto& p = g->pending ? g->pending : g->active;
             os << ",\"slots\":" << p->nSlots << ",\"state_rows\":" << p->nStateRows << ",\"params\":" << p->paramMap.size() << ",\"ops\":" << p->nOps << ",\"code_words\":" << p->code.size()
                << ",\"roots\":" << p->rootIds.size() << ",\"pipeline_stages\":" << p->pipeW;
+            // the group's mix channels for any nOut past MAX_OUT_CHANNELS are the ones below nOut (DESIGN.md section 3), of the program
+            // the last block rendered (a queued program takes over at the next block; before the first block, the queued one's)
+            os << ",\"mix_channels\":[";
+            const std::vector<int> mc = mixChannels(*g, g->active ? *g->active : *p, (size_t) 1 << 30);
+            for (size_t i = 0; i < mc.size(); ++i) os << (i ? "," : "") << mc[i];
+            os << "]";
             if (p->specJob) {
                 const int st = p->specJob->state.load(std::memory_order_acquire);
                 os << ",\"spec_state\":" << st << ",\"spec_cubin_bytes\":" << (st > 0 ? p->specJob->kernel.cubin.size() : 0);
@@ -2241,10 +2254,11 @@ int Engine::compile(Group& g, int nIn, std::shared_ptr<Program>& out) {
 
 // ---------------------------------------------------------------------------------------------------------
 // process
-int Engine::ensureBuffers(size_t nIn, size_t nOut, bool perVoiceIn, bool materialise) {
+int Engine::ensureBuffers(size_t nIn, size_t nOut, bool perVoiceIn, bool materialise, size_t wideRows, size_t wideOutRows) {
     size_t tiles = 0;
     for (auto& g : groups_) tiles += (size_t) g->nTiles();
-    const size_t pf = std::max<size_t>(1, tiles) * nOut * blockSize_;
+    const bool wide = nOut > (size_t) MAX_OUT_CHANNELS;
+    const size_t pf = wide ? std::max<size_t>(1, wideRows) * blockSize_ : std::max<size_t>(1, tiles) * nOut * blockSize_;
     if (pf > partialFloats_) {
         dsync();
         if (dPartial_) dfree(dPartial_);
@@ -2259,6 +2273,37 @@ int Engine::ensureBuffers(size_t nIn, size_t nOut, bool perVoiceIn, bool materia
             if (dOutVoice_) dfree(dOutVoice_);
             if (!cuda(dmalloc((void**) &dOutVoice_, sizeof(float) * of), "cudaMalloc voice out")) return rc::CudaError;
             outVoiceFloats_ = of;
+            wide_.outZeroValid = false;
+        }
+        const size_t cf = wide ? std::max<size_t>(1, wideOutRows) * blockSize_ : 0;
+        if (cf > outCompactFloats_) {
+            dsync();
+            if (dOutCompact_) dfree(dOutCompact_);
+            if (!cuda(dmalloc((void**) &dOutCompact_, sizeof(float) * cf), "cudaMalloc compact voice out")) { dOutCompact_ = nullptr; outCompactFloats_ = 0; return rc::CudaError; }
+            outCompactFloats_ = cf;
+        }
+    }
+    // the mix bus and its mapped host copy grow to the widest nOut used (elem_b200_mix_device: the pointer moves then)
+    const size_t mf = nOut * blockSize_;
+    if (mf > mixFloats_) {
+        dsync();
+        if (dMix_) dfree(dMix_);
+        dMix_ = nullptr; mixFloats_ = 0;
+        if (!cuda(dmalloc((void**) &dMix_, sizeof(float) * mf), "cudaMalloc mix")) return rc::CudaError;
+        dmemset(dMix_, 0, sizeof(float) * mf);
+        mixFloats_ = mf;
+        if (hMixHost_) {   // a failure here only disables the fast hand-over, as at construction
+            cudaFreeHost(hMixHost_);
+            hMixHost_ = nullptr; hMixFlag_ = nullptr; dMixHostAlias_ = nullptr; dMixFlagAlias_ = nullptr;
+            void* d = nullptr;
+            if (cudaHostAlloc((void**) &hMixHost_, sizeof(float) * mf + 64, cudaHostAllocMapped) == cudaSuccess) {
+                std::memset(hMixHost_, 0, sizeof(float) * mf + 64);
+                if (cudaHostGetDevicePointer(&d, hMixHost_, 0) == cudaSuccess) {
+                    hMixFlag_ = reinterpret_cast<volatile uint32_t*>(hMixHost_ + mf);
+                    dMixHostAlias_ = static_cast<float*>(d);
+                    dMixFlagAlias_ = reinterpret_cast<uint32_t*>(dMixHostAlias_ + mf);
+                } else { cudaFreeHost(hMixHost_); hMixHost_ = nullptr; cudaGetLastError(); }
+            } else { hMixHost_ = nullptr; cudaGetLastError(); }
         }
     }
     if (perVoiceIn && nIn) { if (!voiceInDevicePtr(nIn)) return rc::CudaError; }
@@ -2301,7 +2346,13 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
     if (planOnly_ && !planDryRun_) return fail(rc::CudaError, "plan-only runtime (no CUDA device): rendering is impossible, there is no CPU fallback");
     const bool dry = planOnly_;
     dsetdev();
-    if (numSamples > (size_t) blockSize_ || nOut > (size_t) MAX_OUT_CHANNELS) return fail(rc::BadArgument, "numSamples > blockSize or too many output channels");
+    if (numSamples > (size_t) blockSize_ || nOut > (size_t) MAX_WIDE_OUT_CHANNELS) return fail(rc::BadArgument, "numSamples > blockSize or too many output channels");
+    // Past MAX_OUT_CHANNELS the mix bus is compact (DESIGN.md section 3): per channel, only the partial rows of the groups that aim at it
+    const bool wide = nOut > (size_t) MAX_OUT_CHANNELS;
+    if (wide && mix && allReduce && peerAttached_ && peer_.world > 1)
+        return fail(rc::BadArgument, "the cross-GPU mix bus carries at most 8 output channels (its exchange buffer is sized at export)");
+    if (wide && offlineOut_) return fail(rc::BadArgument, "renderOffline: at most 8 output channels");
+    if (!wide && materialise && !offlineOut_) wide_.outZeroValid = false;   // K1 writes [voice][nOut] in the dense layout
 
     const size_t key[6] = {nIn, nOut, numSamples, (size_t) perVoiceIn, (size_t) materialise | ((size_t) (uintptr_t) offlineOut_ << 1), (size_t) mix | ((size_t) offlineStride_ << 1)};
     if (steadyValid_ && !dry && std::memcmp(key, steadyKey_, sizeof key) == 0) {
@@ -2309,13 +2360,16 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
             BatchBuffers& bb = batch_[sb.key];
             auto ev = timedBegin();
             if (!cuda(sb.pipeStages >= 1
-                          ? launch_render_groups_pipe(bb.dDescs, bb.dTileStart, sb.nGroups, sb.totalTiles, sb.pipeStages, sb.maxSlots, (int) nOut, sb.maxState, sb.maxParams, sampleTime_, offlineOut_ ? offlineOffset_ : 0, stream_, opt_.niter)
-                          : launch_render_groups(bb.dDescs, bb.dTileStart, sb.nGroups, sb.totalTiles, sb.L, sb.maxSlots, (int) nOut, sb.maxState, sb.maxParams, sb.wpc, sampleTime_, offlineOut_ ? offlineOffset_ : 0, stream_, opt_.niter),
+                          ? launch_render_groups_pipe(bb.dDescs, bb.dTileStart, sb.nGroups, sb.totalTiles, sb.pipeStages, sb.maxSlots, sb.smemOut, sb.maxState, sb.maxParams, sampleTime_, offlineOut_ ? offlineOffset_ : 0, stream_, opt_.niter)
+                          : launch_render_groups(bb.dDescs, bb.dTileStart, sb.nGroups, sb.totalTiles, sb.L, sb.maxSlots, sb.smemOut, sb.maxState, sb.maxParams, sb.wpc, sampleTime_, offlineOut_ ? offlineOffset_ : 0, stream_, opt_.niter),
                       "render groups kernel launch")) return rc::CudaError;
             if (timeKernels_) { cudaEventRecord(ev.second, stream_); timedEvents_.push_back(ev); }
             ++launches_;
         }
-        if (mix) {
+        if (wide) {
+            const int rw = launchWide(nOut, numSamples, materialise, mix);
+            if (rw != rc::Ok) return rw;
+        } else if (mix) {
             auto ev = timedBegin();
             if (!cuda(launch_mix_reduce(dPartial_, dMix_, dMixScratch_, dMixTickets_, steadyTiles_, (int) nOut, blockSize_, (int) numSamples, stream_, takeDeliver()), "mix reduce launch")) return rc::CudaError;
             if (timeKernels_) { cudaEventRecord(ev.second, stream_); timedMixEvents_.push_back(ev); }
@@ -2350,19 +2404,73 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
             } else g.active->nIn = (int) nIn;
         }
     }
-    int r = ensureBuffers(nIn, nOut, perVoiceIn, materialise);
+    // Wide path: each group's mix channels, the run of compact partial rows it owns ([tile][mix channel]) and its run of compact
+    // per-voice output rows ([voice][mix channel]), in engine order
+    std::vector<std::vector<int>> wideCh;
+    std::vector<size_t> wideRowBase, wideOutBase;
+    size_t wideRows = 0, wideOutRows = 0;
+    if (wide) {
+        wideCh.resize(groups_.size()); wideRowBase.assign(groups_.size(), 0); wideOutBase.assign(groups_.size(), 0);
+        for (size_t gi = 0; gi < groups_.size(); ++gi) {
+            const Group& g = *groups_[gi];
+            if (g.active && g.nTiles()) wideCh[gi] = mixChannels(g, *g.active, nOut);
+            wideRowBase[gi] = wideRows; wideOutBase[gi] = wideOutRows;
+            wideRows += (size_t) g.nTiles() * wideCh[gi].size();
+            wideOutRows += (size_t) g.nv * wideCh[gi].size();
+        }
+        // the row list of channel c (CSR): groups in engine order, tiles in order; then K2's tile groups of each list
+        WidePlan& w = wide_;
+        std::vector<int> rowPtr(nOut + 1, 0);
+        for (size_t gi = 0; gi < groups_.size(); ++gi)
+            for (int c : wideCh[gi]) rowPtr[c + 1] += groups_[gi]->nTiles();
+        for (size_t c = 0; c < nOut; ++c) rowPtr[c + 1] += rowPtr[c];
+        w.rows.assign(rowPtr[nOut], 0);
+        std::vector<int> pos(rowPtr.begin(), rowPtr.end() - 1);
+        for (size_t gi = 0; gi < groups_.size(); ++gi) {
+            const int nC = (int) wideCh[gi].size(), nT = groups_[gi]->nTiles();
+            for (int k = 0; k < nC; ++k)
+                for (int t = 0; t < nT; ++t) w.rows[pos[wideCh[gi][k]]++] = (int) wideRowBase[gi] + t * nC + k;
+        }
+        w.segs.clear(); w.nScratch = 0;
+        for (size_t c = 0; c < nOut; ++c) {
+            const int n = rowPtr[c + 1] - rowPtr[c];
+            const int G = n == 0 ? 1 : std::min(MIX_REDUCE_MAX_GROUPS, (n + 255) / 256);
+            const int per = ((n + G - 1) / G + 31) / 32 * 32;
+            const int sc = G > 1 ? w.nScratch : -1;
+            if (G > 1) w.nScratch += G;
+            for (int k = 0; k < G; ++k) {
+                const int b = std::min(n, k * per), e = std::min(n, k * per + per);
+                w.segs.push_back(WideSeg{(int) c, rowPtr[c] + b, e - b, G, k, sc});
+            }
+        }
+        // K2w takes the segments of fewer than WIDE_BIG_ROWS rows first (a warp each), then the larger ones (a CTA each)
+        w.nSmall = (int) (std::stable_partition(w.segs.begin(), w.segs.end(), [](const WideSeg& sg) { return sg.rowCount < WIDE_BIG_ROWS; }) - w.segs.begin());
+        w.dstRow.clear();
+        if (materialise)
+            for (size_t gi = 0; gi < groups_.size(); ++gi) {
+                const Group& g = *groups_[gi];
+                for (int v = 0; v < (wideCh[gi].empty() ? 0 : g.nv); ++v)
+                    for (int c : wideCh[gi]) w.dstRow.push_back((g.v0 + v) * (int) nOut + c);
+            }
+    }
+    int r = ensureBuffers(nIn, nOut, perVoiceIn, materialise, wideRows, wideOutRows);
     if (r != rc::Ok) return r;
+    if (wide && !dry) {
+        r = uploadWidePlan();
+        if (r != rc::Ok) return r;
+    }
 
     int tileBase = 0;
     std::map<int, std::vector<LaunchParams>> buckets;   // tile width -> single-stage groups launched together
     for (auto& gp : groups_) {
         Group& g = *gp;
+        const size_t gi = (size_t) (&gp - groups_.data());
         const int nTiles = g.nTiles();
         if (!g.active || nTiles == 0) { allSteady = false; }
         if (!g.active || nTiles == 0) {
             // no render sequence yet: outputs are silence (Runtime.h:287-289 leaves the host buffers untouched;
             // we define the voice's contribution as zero)
-            if (nTiles && mix) dmemset(dPartial_ + (size_t) tileBase * nOut * blockSize_, 0, sizeof(float) * (size_t) nTiles * nOut * blockSize_);
+            if (nTiles && mix && !wide) dmemset(dPartial_ + (size_t) tileBase * nOut * blockSize_, 0, sizeof(float) * (size_t) nTiles * nOut * blockSize_);
             if (materialise && dOutVoice_ && !offlineOut_) dmemset(dOutVoice_ + (size_t) g.v0 * nOut * blockSize_, 0, sizeof(float) * (size_t) g.nv * nOut * blockSize_);
             tileBase += nTiles;
             continue;
@@ -2376,23 +2484,27 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
         P.rows = g.dRows;
         P.inShared = (!perVoiceIn && nIn) ? dInShared_ : nullptr;
         P.inVoice = (perVoiceIn && nIn) ? dInVoice_ : nullptr;
-        float* const voiceOut = offlineOut_ ? offlineOut_ : dOutVoice_;
+        // wide: the group's own runs of compact rows, per-voice I/O indexed from its first voice (voice0 = 0)
+        const std::vector<int>* const gch = wide ? &wideCh[gi] : nullptr;
+        float* const voiceOut = wide ? (gch->empty() ? nullptr : dOutCompact_ + wideOutBase[gi] * blockSize_) : (offlineOut_ ? offlineOut_ : dOutVoice_);
+        float* const partialOut = wide ? (gch->empty() ? nullptr : dPartial_ + wideRowBase[gi] * blockSize_) : dPartial_;
+        if (wide && P.inVoice) P.inVoice += (size_t) g.v0 * nIn * blockSize_;
         P.outVoice = materialise ? voiceOut : nullptr;
-        P.mixPartial = mix ? dPartial_ : nullptr;
+        P.mixPartial = mix ? partialOut : nullptr;
         P.nStateEntries = (int) p.stateMap.size();
         P.nStateRows = p.nStateRows;
         P.nSlots = p.nSlots;
         P.Vpad = g.Vpad;
         P.nv = g.nv;
-        P.voice0 = g.v0;
+        P.voice0 = wide ? 0 : g.v0;
         P.tileWidth = g.tileWidth;
         P.numSamples = (int) numSamples;
         P.blockSize = blockSize_;
         P.nIn = (int) nIn;
-        P.nOut = (int) nOut;
+        P.nOut = wide ? (int) gch->size() : (int) nOut;
         P.inStride = blockSize_;
         P.outStride = offlineOut_ ? offlineStride_ : blockSize_;
-        P.tileBase = tileBase;
+        P.tileBase = wide ? 0 : tileBase;
         uint32_t runMask = 0;
         for (size_t ri = 0; ri < p.rootIds.size(); ++ri) {
             auto it = g.nodes.find(p.rootIds[ri]);
@@ -2402,7 +2514,12 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
             const bool chanOk = rn.channel >= 0 && (size_t) rn.channel < nOut;                // GraphRenderSequence.h:214-219
             if (stillRunning && chanOk) runMask |= (1u << ri);
             if (rn.fade.on()) runMask |= (1u << (16 + ri));                                   // promoteTapBuffers: :200-205
-            P.roots[ri] = RootDyn{rn.fade.current, rn.fade.step, rn.fade.target, rn.channel};
+            int chan = rn.channel;
+            if (wide) {   // the compact index of the channel among the group's mix channels
+                const auto at = std::lower_bound(gch->begin(), gch->end(), chan);
+                chan = (chanOk && at != gch->end() && *at == chan) ? (int) (at - gch->begin()) : -1;
+            }
+            P.roots[ri] = RootDyn{rn.fade.current, rn.fade.step, rn.fade.target, chan};
             if (rn.fade.current != rn.fade.target) allSteady = false;        // the descriptor changes while a root fades
         }
         if (!p.evNodes.empty() || !p.dynNodes.empty() || g.codeDirty || g.pending) allSteady = false;
@@ -2440,7 +2557,7 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
         // launch geometry: spread warps over the SMs first, then stack them
         int wpc = opt_.warpsPerCta;
         if (wpc <= 0) wpc = nTiles >= smCount_ * 8 ? 4 : (nTiles >= smCount_ * 4 ? 2 : 1);
-        const size_t perWarp = render_smem_bytes(p.nSlots, (int) nOut, p.nStateRows, (int) p.paramMap.size(), 1, g.tileWidth, opt_.niter);
+        const size_t perWarp = render_smem_bytes(p.nSlots, P.nOut, p.nStateRows, (int) p.paramMap.size(), 1, g.tileWidth, opt_.niter);
         while (wpc > 1 && perWarp * wpc > 200 * 1024) wpc >>= 1;
         if (perWarp > 220 * 1024) return fail(rc::InvariantViolation, "graph state does not fit in shared memory");
         const size_t nStages = std::max<size_t>(1, p.stages.size());
@@ -2458,7 +2575,7 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
             const bool last = stg + 1 == nStages;
             P.code = p.dCode + (p.stages.empty() ? 0 : p.stages[stg].codeOffset);
             P.outVoice = (last && materialise) ? voiceOut + (offlineOut_ ? offlineOffset_ : 0) : nullptr;   // outputs and taps belong to the last stage
-            P.mixPartial = (last && mix) ? dPartial_ : nullptr;
+            P.mixPartial = (last && mix) ? partialOut : nullptr;
             std::pair<cudaEvent_t, cudaEvent_t> ev{nullptr, nullptr};
             if (timeKernels_) {
                 if (!eventPool_.empty()) { ev = eventPool_.back(); eventPool_.pop_back(); }
@@ -2491,10 +2608,10 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
                     epi.active = true;
                     epi.running = ((runMask >> p.fusedRoot) & 1u) != 0;
                     epi.gain0 = rd.gain0; epi.step = rd.step; epi.target = rd.target; epi.channel = rd.channel;
-                    epi.nOut = (int) nOut; epi.blockSize = blockSize_;
-                    epi.mixPartial = mix ? dPartial_ : nullptr; epi.tileBase = tileBase;
+                    epi.nOut = P.nOut; epi.blockSize = blockSize_;
+                    epi.mixPartial = mix ? partialOut : nullptr; epi.tileBase = P.tileBase;
                     epi.outVoice = materialise ? voiceOut + (offlineOut_ ? offlineOffset_ : 0) : nullptr;
-                    epi.voice0 = g.v0; epi.outStride = P.outStride; epi.outOffset = 0;
+                    epi.voice0 = P.voice0; epi.outStride = P.outStride; epi.outOffset = 0;
                 }
                 int offset = 0;
                 while (offset < (int) numSamples) {
@@ -2533,9 +2650,10 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
         auto& descs = kv.second;
         const int L = kv.first % PIPE_BUCKET;
         std::vector<int> tileStart(descs.size());
-        int total = 0, maxSlots = 1, maxState = 0, maxParams = 0, pipeStages = 0;
+        int total = 0, maxSlots = 1, maxState = 0, maxParams = 0, pipeStages = 0, smemOut = 0;
         for (size_t i = 0; i < descs.size(); ++i) {
             tileStart[i] = total;
+            smemOut = std::max(smemOut, descs[i].nOut);   // = nOut unless wide
             total += (descs[i].nv + L - 1) / L;
             maxSlots = std::max(maxSlots, descs[i].nSlots);
             maxState = std::max(maxState, descs[i].nStateRows);
@@ -2561,17 +2679,17 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
         }
         int wpc = opt_.warpsPerCta;
         if (wpc <= 0) wpc = total >= smCount_ * 8 ? 4 : (total >= smCount_ * 4 ? 2 : 1);
-        while (wpc > 1 && render_smem_bytes(maxSlots, (int) nOut, maxState, maxParams, wpc, L, opt_.niter) > 200 * 1024) wpc >>= 1;
+        while (wpc > 1 && render_smem_bytes(maxSlots, smemOut, maxState, maxParams, wpc, L, opt_.niter) > 200 * 1024) wpc >>= 1;
         std::pair<cudaEvent_t, cudaEvent_t> ev{nullptr, nullptr};
         if (timeKernels_) {
             if (!eventPool_.empty()) { ev = eventPool_.back(); eventPool_.pop_back(); }
             else { cudaEventCreate(&ev.first); cudaEventCreate(&ev.second); }
             cudaEventRecord(ev.first, stream_);
         }
-        steadyBuckets_.push_back(SteadyBucket{L, (int) descs.size(), total, maxSlots, maxState, maxParams, wpc, pipeStages, kv.first});
+        steadyBuckets_.push_back(SteadyBucket{L, (int) descs.size(), total, maxSlots, maxState, maxParams, wpc, pipeStages, kv.first, smemOut});
         if (!dry && !cuda(pipeStages >= 1
-                              ? launch_render_groups_pipe(bb.dDescs, bb.dTileStart, (int) descs.size(), total, pipeStages, maxSlots, (int) nOut, maxState, maxParams, sampleTime_, offlineOut_ ? offlineOffset_ : 0, stream_, opt_.niter)
-                              : launch_render_groups(bb.dDescs, bb.dTileStart, (int) descs.size(), total, L, maxSlots, (int) nOut, maxState, maxParams, wpc, sampleTime_, offlineOut_ ? offlineOffset_ : 0, stream_, opt_.niter),
+                              ? launch_render_groups_pipe(bb.dDescs, bb.dTileStart, (int) descs.size(), total, pipeStages, maxSlots, smemOut, maxState, maxParams, sampleTime_, offlineOut_ ? offlineOffset_ : 0, stream_, opt_.niter)
+                              : launch_render_groups(bb.dDescs, bb.dTileStart, (int) descs.size(), total, L, maxSlots, smemOut, maxState, maxParams, wpc, sampleTime_, offlineOut_ ? offlineOffset_ : 0, stream_, opt_.niter),
                   "render groups kernel launch")) return rc::CudaError;
         if (timeKernels_) { cudaEventRecord(ev.second, stream_); timedEvents_.push_back(ev); }
         ++launches_;
@@ -2584,7 +2702,12 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
         ++peerEpoch_;
         mixOut = peer_.own;
     }
-    if (mix) {
+    if (wide) {
+        if (!dry) {
+            const int rw = launchWide(nOut, numSamples, materialise, mix);
+            if (rw != rc::Ok) return rw;
+        }
+    } else if (mix) {
         if (tileBase > 0) {
             auto ev = timedBegin();
             if (!dry && !cuda(launch_mix_reduce(dPartial_, mixOut, dMixScratch_, dMixTickets_, tileBase, (int) nOut, blockSize_, (int) numSamples, stream_, exchange ? HostDeliver{} : takeDeliver()), "mix reduce launch")) return rc::CudaError;
@@ -2605,6 +2728,81 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
     steadyTiles_ = tileBase;
     curNOut_ = nOut;
     sampleTime_ += (int64_t) numSamples;   // wasm/Main.cpp:217
+    return rc::Ok;
+}
+
+std::vector<int> Engine::mixChannels(const Group& g, const Program& p, size_t nOut) const {
+    std::vector<int> ch;
+    for (int32_t id : p.rootIds) {
+        auto it = g.nodes.find(id);
+        if (it == g.nodes.end()) continue;
+        const int c = it->second.channel;
+        if (c >= 0 && (size_t) c < nOut) ch.push_back(c);
+    }
+    std::sort(ch.begin(), ch.end());
+    ch.erase(std::unique(ch.begin(), ch.end()), ch.end());
+    return ch;
+}
+
+// Upload what changed of the wide plan (row lists, segments, output rows) and grow K2w's scratch and tickets.
+int Engine::uploadWidePlan() {
+    WidePlan& w = wide_;
+    auto upload = [&](auto& dev, size_t& cap, const auto& host, auto& shadow, const char* what) -> bool {
+        typedef typename std::remove_reference<decltype(host)>::type::value_type T;
+        const size_t n = std::max<size_t>(1, host.size());
+        if (n > cap) {
+            dsync();
+            if (dev) dfree(dev);
+            dev = nullptr; cap = 0; shadow.clear();
+            if (!cuda(dmalloc((void**) &dev, n * 2 * sizeof(T)), what)) { dev = nullptr; return false; }
+            cap = n * 2;
+        }
+        const size_t bytes = host.size() * sizeof(T);
+        if (shadow.size() == bytes / sizeof(shadow[0]) && std::memcmp(shadow.data(), host.data(), bytes) == 0) return true;
+        if (bytes && !cuda(dmemcpy(dev, host.data(), bytes, cudaMemcpyHostToDevice), what)) return false;
+        shadow.resize(bytes / sizeof(shadow[0]));
+        if (bytes) std::memcpy(shadow.data(), host.data(), bytes);
+        return true;
+    };
+    if (!upload(w.dRows, w.capRows, w.rows, w.upRows, "upload wide row lists")) return rc::CudaError;
+    if (!upload(w.dSegs, w.capSegs, w.segs, w.upSegs, "upload wide segments")) return rc::CudaError;
+    if (!upload(w.dDst, w.capDst, w.dstRow, w.upDst, "upload wide output rows")) return rc::CudaError;
+    if ((size_t) w.nScratch > wideScratchRows_) {
+        dsync();
+        if (dWideScratch_) dfree(dWideScratch_);
+        if (dWideTickets_) dfree(dWideTickets_);
+        dWideScratch_ = nullptr; dWideTickets_ = nullptr; wideScratchRows_ = 0;
+        const size_t rowsCap = (size_t) w.nScratch * 2, tick = rowsCap * ((blockSize_ + 31) / 32);
+        if (!cuda(dmalloc((void**) &dWideScratch_, sizeof(float) * rowsCap * blockSize_), "cudaMalloc wide mix scratch")) return rc::CudaError;
+        if (!cuda(dmalloc((void**) &dWideTickets_, sizeof(unsigned int) * tick), "cudaMalloc wide mix tickets")) return rc::CudaError;
+        if (!cuda(dmemset(dWideTickets_, 0, sizeof(unsigned int) * tick), "memset wide mix tickets")) return rc::CudaError;
+        wideScratchRows_ = rowsCap;
+    }
+    return rc::Ok;
+}
+
+// The device half of a wide block after K1 / K3: per-voice outputs scattered to [voice][nOut] (every other channel zero), then K2w,
+// which also hands the mix bus to the host.
+int Engine::launchWide(size_t nOut, size_t numSamples, bool materialise, bool mix) {
+    WidePlan& w = wide_;
+    if (materialise && dOutVoice_) {
+        // The channels no root of a voice aims at stay zero from block to block: the whole buffer is cleared only when the rows the
+        // scatter writes (or nOut) changed, or something else wrote it since (the narrow path, a reallocation).
+        if (!w.outZeroValid || w.outZeroNOut != nOut || w.outZeroRows != w.dstRow) {
+            if (!cuda(dmemset(dOutVoice_, 0, sizeof(float) * (size_t) numVoices_ * nOut * blockSize_), "memset voice out")) return rc::CudaError;
+            w.outZeroValid = true; w.outZeroNOut = nOut; w.outZeroRows = w.dstRow;
+        }
+        if (!cuda(launch_voice_out_scatter(dOutCompact_, w.dDst, (int) w.dstRow.size(), dOutVoice_, blockSize_, (int) numSamples, stream_), "voice out scatter launch")) return rc::CudaError;
+        if (!w.dstRow.empty() && numSamples) ++launches_;
+    }
+    if (mix) {
+        auto ev = timedBegin();
+        const int nBig = (int) w.segs.size() - w.nSmall;
+        if (!cuda(launch_mix_reduce_wide(dPartial_, w.dRows, w.dSegs, w.nSmall, nBig, (int) nOut, dMix_, dWideScratch_, dWideTickets_, blockSize_,
+                                         (int) numSamples, stream_, takeDeliver()), "wide mix reduce launch")) return rc::CudaError;
+        if (timeKernels_) { cudaEventRecord(ev.second, stream_); timedMixEvents_.push_back(ev); }
+        launches_ += (w.nSmall > 0) + (nBig > 0);
+    }
     return rc::Ok;
 }
 

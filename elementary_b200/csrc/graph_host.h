@@ -302,7 +302,7 @@ private:
     std::pair<cudaEvent_t, cudaEvent_t> timedBegin();
 
     // I/O staging
-    float* dMix_ = nullptr;          // [MAX_OUT][blockSize]
+    float* dMix_ = nullptr;          // [max(MAX_OUT, widest nOut so far)][blockSize]
     float* dMixScratch_ = nullptr;   // K2 group sums [MIX_REDUCE_MAX_GROUPS][MAX_OUT][blockSize]
     unsigned int* dMixTickets_ = nullptr;
     float* dPartial_ = nullptr; size_t partialFloats_ = 0;
@@ -310,7 +310,7 @@ private:
     float* dInVoice_ = nullptr; size_t inVoiceFloats_ = 0;
     float* dInShared_ = nullptr; size_t inSharedFloats_ = 0;
     float* hPinned_ = nullptr; size_t pinnedFloats_ = 0;
-    // Host delivery of the mix bus (kernels.h HostDeliver): mapped pinned [MAX_OUT][blockSize] floats + the sequence word behind them.
+    // Host delivery of the mix bus (kernels.h HostDeliver): mapped pinned [mixFloats_] floats + the sequence word behind them.
     // process() arms it for the block it enqueues and polls the word instead of D2H copy + stream synchronize.
     float* hMixHost_ = nullptr; float* dMixHostAlias_ = nullptr;
     volatile uint32_t* hMixFlag_ = nullptr; uint32_t* dMixFlagAlias_ = nullptr;
@@ -327,12 +327,36 @@ private:
     // every group steady — no queued program, nothing dirty, all root fades settled, no event mirrors to advance — and the call has the
     // same shape, the next block re-launches the cached buckets (the descriptors on the device are still right; the sample clock is a
     // kernel argument) without walking the groups.  Any instruction batch, gc, option or resource change invalidates it.
-    struct SteadyBucket { int L, nGroups, totalTiles, maxSlots, maxState, maxParams, wpc, pipeStages, key; };
+    struct SteadyBucket { int L, nGroups, totalTiles, maxSlots, maxState, maxParams, wpc, pipeStages, key, smemOut; };
     static constexpr int PIPE_BUCKET = 1000;   // bucket key = tile width (+ PIPE_BUCKET for pipelined one-voice programs)
     std::vector<SteadyBucket> steadyBuckets_;
     bool steadyValid_ = false;
     size_t steadyKey_[6] = {0, 0, 0, 0, 0, 0};
     int steadyTiles_ = 0;
+    // Wide mix bus (nOut > MAX_OUT_CHANNELS, DESIGN.md section 3): each voice group writes compact partial rows for the channels its
+    // roots aim at only (mix channels, ascending), per-voice outputs go to a compact [voice][mix channel] buffer and are scattered to
+    // [voice][nOut]; K2w reduces each channel over its own row list.  Rebuilt by every slow pass; the device copies are re-uploaded
+    // only when they change, so the steady-state fast path relaunches K2w on them as they stand.
+    struct WidePlan {
+        std::vector<int> rows;            // CSR row lists of the channels, concatenated in channel order
+        std::vector<WideSeg> segs;        // K2w segments
+        std::vector<int> dstRow;          // compact per-voice output row -> row of [voice][nOut]
+        int nScratch = 0;                 // scratch / ticket rows of the channels with more than one tile group
+        int* dRows = nullptr; size_t capRows = 0;
+        WideSeg* dSegs = nullptr; size_t capSegs = 0;
+        int* dDst = nullptr; size_t capDst = 0;
+        std::vector<int> upRows, upDst; std::vector<char> upSegs;   // what the device copies hold
+        int nSmall = 0;                   // segs[0, nSmall) have fewer than WIDE_BIG_ROWS rows
+        // the per-voice output buffer is zero outside outZeroRows (rows of [voice][outZeroNOut]) since its last clear
+        bool outZeroValid = false; size_t outZeroNOut = 0; std::vector<int> outZeroRows;
+    } wide_;
+    float* dWideScratch_ = nullptr; unsigned int* dWideTickets_ = nullptr; size_t wideScratchRows_ = 0;
+    float* dOutCompact_ = nullptr; size_t outCompactFloats_ = 0;
+    size_t mixFloats_ = 0;                // dMix_ and the mapped host-delivery buffer hold this many floats
+    int uploadWidePlan();
+    int launchWide(size_t nOut, size_t numSamples, bool materialise, bool mix);
+    // the mix channels of a program: distinct channels in [0, nOut) of all its roots, running or fading, ascending
+    std::vector<int> mixChannels(const Group& g, const Program& p, size_t nOut) const;
     float* offlineOut_ = nullptr; int offlineStride_ = 0, offlineOffset_ = 0;   // renderOffline: where materialised outputs go instead of dOutVoice_
 
     // K4 state
@@ -376,7 +400,7 @@ private:
     int compile(Group& g, int nIn, std::shared_ptr<Program>& out);
     void traverse(Group& g, std::set<int32_t>& visited, std::vector<int32_t>& order, int32_t n);
     int chooseTileWidth(int nv) const;
-    int ensureBuffers(size_t nIn, size_t nOut, bool perVoiceIn, bool materialise);
+    int ensureBuffers(size_t nIn, size_t nOut, bool perVoiceIn, bool materialise, size_t wideRows = 0, size_t wideOutRows = 0);
     friend struct Compiler;
 };
 

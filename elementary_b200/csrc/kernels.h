@@ -38,6 +38,24 @@ struct HostDeliver {
 cudaError_t launch_mix_reduce(const float* partial, float* out, float* scratch, unsigned int* tickets, int nTiles, int nOut, int blockSize,
                               int numSamples, cudaStream_t stream, HostDeliver hd = HostDeliver{});
 
+// K2w (mix_wide_kernel.cu): the mix bus for nOut > MAX_OUT_CHANNELS from COMPACT partial rows [row][blockSize].  Channel c sums its row
+// list rows[rowPtr_c ...] with K2's tree; a segment is one tile group of one channel.  Every channel in [0, nOut) has at least one
+// segment (a channel without rows has one empty segment, which writes +0.0).
+constexpr int MAX_WIDE_OUT_CHANNELS = 4096;   // output channels of the compact mix bus; a call with more returns -2
+struct WideSeg {
+    int channel;
+    int rowBegin, rowCount;   // the group's rows: rows[rowBegin .. rowBegin + rowCount)
+    int groups, group;        // G_c and this segment's index in it
+    int scratch;              // G_c > 1: first of the channel's G_c scratch rows [blockSize] and ticket rows [ceil(blockSize / 32)]; else -1
+};
+// segs: the nSmall segments of fewer than WIDE_BIG_ROWS rows (a warp each), then the nBig larger ones (a CTA of 32 warps each).
+constexpr int WIDE_BIG_ROWS = 128;
+cudaError_t launch_mix_reduce_wide(const float* partial, const int* rows, const WideSeg* segs, int nSmall, int nBig, int nOut, float* out,
+                                   float* scratch, unsigned int* tickets, int blockSize, int numSamples, cudaStream_t stream,
+                                   HostDeliver hd = HostDeliver{});
+// Per-voice outputs of the wide path: compact row r [blockSize] -> row dstRow[r] of out ([voice][nOut][blockSize]), numSamples samples.
+cudaError_t launch_voice_out_scatter(const float* compact, const int* dstRow, int nRows, float* out, int blockSize, int numSamples, cudaStream_t stream);
+
 // K4: the one collective of the path (SURVEY.md §8e) as our own kernel over NVLink/NVSwitch peer memory: K2 leaves this rank's
 // partial mix bus in PeerMix::own; world-1 CTAs each push it into one peer's buffer as (sample, epoch) pairs, then every CTA waits for the
 // pairs of all sources to arrive in its OWN buffer and sums a share of the samples in rank order — one launch, deterministic, no NCCL

@@ -31,6 +31,9 @@ extern "C" {
 
 typedef struct elem_b200_runtime elem_b200_runtime;
 
+/* Output channels of elem_b200_process / _process_voices / _enqueue_block (the mix bus past 8 channels is compact, see process). */
+#define ELEM_B200_MAX_OUT_CHANNELS 4096
+
 /* Runtime<float>::Runtime(double sampleRate, int blockSize)  — runtime/elem/Runtime.h:44,158-166.
  * New here: numVoices independent instances living on CUDA device `device`. */
 elem_b200_runtime* elem_b200_create(double sampleRate, int blockSize, int numVoices, int device);
@@ -84,7 +87,12 @@ int elem_b200_set_path_per_voice(elem_b200_runtime* rt, int32_t nodeId, const ch
  * rank must make the call for every block.
  * userData: NULL, or — as every reference host passes it (wasm/Main.cpp:206-215) — a pointer to the int64 sample
  * time of the block's first sample, read by the `time` and `metro` nodes (wasm/SampleTime.h:19, Metro.h:44).
- * With NULL the engine keeps the clock itself (+= numSamples per call, like wasm/Main.cpp:217). */
+ * With NULL the engine keeps the clock itself (+= numSamples per call, like wasm/Main.cpp:217).
+ * OUTPUT CHANNELS: nOut <= 4096 (ELEM_B200_MAX_OUT_CHANNELS); more returns -2.  A root aimed outside [0, nOut) does not run and its
+ * nodes keep their state, as in the reference.  Up to 8 channels the mix is K2's fixed summation tree over all tiles (DESIGN.md §4).
+ * Past 8 the mix bus is compact: each voice group writes partial rows only for the channels its roots aim at, and channel c is K2's
+ * tree over its own rows — the groups that write c in engine order, their tiles in order (K2w, DESIGN.md §3-4); still deterministic
+ * run to run.  Past 8 channels peers may not be attached with the cross-GPU sum requested (-2). */
 int elem_b200_process(elem_b200_runtime* rt, const float* const* in, size_t nIn,
                       float* const* out, size_t nOut, size_t numSamples, void* userData);
 
@@ -93,12 +101,13 @@ void elem_b200_set_current_time(elem_b200_runtime* rt, int64_t sampleTime);
 int64_t elem_b200_current_time(elem_b200_runtime* rt);
 
 /* Voice-major variant for per-voice I/O and parity tests: in = [voice][nIn][numSamples] or NULL,
- * outVoices = [voice][nOut][numSamples] or NULL, mix = [nOut][numSamples] or NULL (all host memory). */
+ * outVoices = [voice][nOut][numSamples] or NULL, mix = [nOut][numSamples] or NULL (all host memory).
+ * nOut <= 4096 with the mix order of elem_b200_process; past 8 channels a voice's channels that none of its roots aim at are zero. */
 int elem_b200_process_voices(elem_b200_runtime* rt, const float* in, size_t nIn,
                              float* outVoices, float* mix, size_t nOut, size_t numSamples);
 
 /* Offline rendering (what js/packages/offline-renderer does with process() in a loop; BASELINE config 5): numBlocks full blocks of every
- * voice, per-voice output hostOut[voice][nOut][numBlocks * blockSize] (host memory), no inputs, no mix bus.  Blocks are enqueued back to
+ * voice, per-voice output hostOut[voice][nOut][numBlocks * blockSize] (host memory, nOut <= 8), no inputs, no mix bus.  Blocks are enqueued back to
  * back with no host synchronisation in between; outputs are written by the kernels into device chunk buffers of chunkBlocks blocks
  * (0 = default 32) and copied out on a second stream while the next chunk renders. */
 int elem_b200_render_offline(elem_b200_runtime* rt, size_t nOut, size_t numBlocks, float* hostOut, size_t chunkBlocks);
@@ -106,11 +115,14 @@ int elem_b200_render_offline(elem_b200_runtime* rt, size_t nOut, size_t numBlock
 /* Device-resident stepping for throughput measurement and pipelines that keep audio in HBM: enqueue one block
  * on the engine's stream (no host copies, no synchronisation).  flags: 1 = read per-voice inputs from
  * elem_b200_voice_in_device(), 2 = materialise per-voice outputs, 4 = produce the mix bus, 8 = (with 4, after
- * elem_b200_peer_attach) sum the mix bus over all ranks in place — every rank ends with the mix of the whole voice set. */
+ * elem_b200_peer_attach) sum the mix bus over all ranks in place — every rank ends with the mix of the whole voice set (nOut <= 8).
+ * nOut <= 4096 with the channel rules and mix order of elem_b200_process. */
 int elem_b200_enqueue_block(elem_b200_runtime* rt, size_t nIn, size_t nOut, size_t numSamples, int flags);
 int elem_b200_synchronize(elem_b200_runtime* rt);
-float* elem_b200_mix_device(elem_b200_runtime* rt);                    /* device pointer [8][blockSize] */
-float* elem_b200_voice_out_device(elem_b200_runtime* rt);              /* device pointer [voice][nOut][blockSize] */
+/* Device pointer [nOut][blockSize] holding the mix of the last enqueued block (at least [8][blockSize]).  The buffer grows the first
+ * time a wider nOut is used, so the pointer may MOVE then: fetch it again after a call with a larger nOut than before. */
+float* elem_b200_mix_device(elem_b200_runtime* rt);
+float* elem_b200_voice_out_device(elem_b200_runtime* rt);              /* device pointer [voice][nOut][blockSize]; may move like the mix */
 float* elem_b200_voice_in_device(elem_b200_runtime* rt, size_t nIn);   /* device pointer [voice][nIn][blockSize] */
 float* elem_b200_shared_in_device(elem_b200_runtime* rt, size_t nIn);  /* device pointer [nIn][blockSize] */
 void elem_b200_set_stream(elem_b200_runtime* rt, void* cudaStream);    /* run on a caller-owned cudaStream_t */
@@ -185,7 +197,9 @@ int elem_b200_has_node_type(elem_b200_runtime* rt, const char* type);
  * Returns the bytes needed including the terminating NUL; writes at most cap. */
 int elem_b200_snapshot(elem_b200_runtime* rt, int voice, char* buf, size_t cap);
 
-/* JSON description of voice groups and compiled programs; returns bytes needed. */
+/* JSON description of voice groups and compiled programs; returns bytes needed.  "steady": the next block of the same shape relaunches
+ * cached work without walking the groups.  Per group, "mix_channels": the non-negative root channels of the program the last block
+ * rendered (before the first block, of the queued one) — its mix channels for any nOut past 8 are those below nOut. */
 int elem_b200_describe(elem_b200_runtime* rt, char* buf, size_t cap);
 /* The encoded render program (32-bit words, elementary_b200/csrc/program.h) of the voice group containing `voice`; writes up to
  * `cap` words, returns the program length.  Introspection only (tests; input of per-program kernel specialisation). */
@@ -207,7 +221,7 @@ double elem_b200_take_kernel_time_ms(elem_b200_runtime* rt, uint64_t* count);
 /* Same for the K3 convolver launches, as gathered by the most recent elem_b200_take_kernel_time_ms() call. */
 double elem_b200_last_convolve_time_ms(elem_b200_runtime* rt, uint64_t* count);
 /* Per kernel kind, as gathered by the most recent elem_b200_take_kernel_time_ms() call: ms[4] / counts[4] = summed device ms and
- * launch counts of K1 (render), K2 (mix reduce), K3 (convolver), K4 (cross-GPU mix exchange). */
+ * launch counts of K1 (render), K2 (mix reduce; K2w past 8 output channels), K3 (convolver), K4 (cross-GPU mix exchange). */
 void elem_b200_last_kernel_times(elem_b200_runtime* rt, double* ms4, uint64_t* counts4);
 const char* elem_b200_last_error(elem_b200_runtime* rt);
 /* ReturnCode::describe — runtime/elem/Types.h:62-85 */
