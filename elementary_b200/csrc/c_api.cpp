@@ -201,7 +201,8 @@ int elem_b200_snapshot(elem_b200_runtime* rt, int voice, char* buf, size_t cap) 
 int elem_b200_debug_opprof(elem_b200_runtime* rt, unsigned long long* out128, int reset) {
     if (!rt || !out128) return -1;
     rt->engine->synchronize();
-    return eb::debug_opprof_read(out128, reset != 0) == cudaSuccess ? 0 : -1;
+    if (eb::debug_opprof_read(out128, reset != 0) != cudaSuccess) return -1;
+    return rt->engine->specOpprofRead(out128, reset != 0) ? 0 : -1;     // + specialised kernels compiled with option spec_opprof
 }
 
 int elem_b200_program_words(elem_b200_runtime* rt, int voice, uint32_t* buf, size_t cap) {

@@ -245,6 +245,7 @@ int Engine::setOption(const char* key, double value) {
     else if (k == "specialize_max_words") { opt_.specializeMaxWords = (int) value; }
     else if (k == "specialize_strict") { opt_.specializeStrict = value != 0; }
     else if (k == "spec_minblocks") { opt_.specMinBlocks = (int) value; }
+    else if (k == "spec_opprof") { opt_.specOpprof = value != 0; }
     else if (k == "time_kernels") { timeKernels_ = value != 0 && !planOnly_; }
     else if (k == "fuse_conv_root") { opt_.fuseConvRoot = value != 0; }
     else if (k == "pipeline_stages") { opt_.pipelineStages = std::max(0, std::min((int) value, (int) MAX_PIPE)); }
@@ -340,11 +341,23 @@ long Engine::specializeDryRun(int voice, std::string& log) {
         if (!p) { log = "no compiled program for this voice"; return -1; }
         if (p->stages.size() > 1) { log = "multi-stage programs (convolve) are not specialised"; return -1; }
         SpecKernel k;
-        if (!specialise_compile(p->code, g->tileWidth, opt_.niter, customSource(), k, log, opt_.specMinBlocks)) return -1;
+        if (!specialise_compile(p->code, g->tileWidth, opt_.niter, customSource(), k, log, opt_.specMinBlocks, opt_.specOpprof)) return -1;
         return (long) k.cubin.size();
     }
     log = "voice out of range";
     return -1;
+}
+
+bool Engine::specOpprofRead(unsigned long long* out128, bool reset) {
+    Lock lk(mu_);
+    std::set<const SpecJob*> seen;
+    for (auto& g : groups_) {
+        const auto& p = g->active;
+        if (!p || !p->specJob || !p->specJob->opprof || p->specJob->state.load(std::memory_order_acquire) != 2) continue;
+        if (!seen.insert(p->specJob.get()).second) continue;
+        if (!specialise_opprof_read(p->specJob->kernel, out128, reset)) return false;
+    }
+    return true;
 }
 
 std::vector<uint32_t> Engine::programWords(int voice) const {
@@ -2241,7 +2254,8 @@ int Engine::compile(Group& g, int nIn, std::shared_ptr<Program>& out) {
         if (prog->specJob->state.load(std::memory_order_acquire) < 0)
             return fail(rc::InvariantViolation, "registered node type failed to compile: " + prog->specJob->log);
     } else if (opt_.specialize && !batched && prog->stages.size() <= 1 && (int) prog->code.size() <= opt_.specializeMaxWords) {
-        prog->specJob = specialise_request(prog->code, g.tileWidth, opt_.niter, device_, std::string(), midRangeDense(g.nv) ? 8 : opt_.specMinBlocks);   // NVRTC on the compile-queue thread
+        prog->specJob = specialise_request(prog->code, g.tileWidth, opt_.niter, device_, std::string(), midRangeDense(g.nv) ? 8 : opt_.specMinBlocks,
+                                            opt_.specOpprof);   // NVRTC on the compile-queue thread
         if (opt_.specialize >= 2) {                                                          // synchronous mode: wait for the compiler here
             specialise_wait(*prog->specJob);
             if (prog->specJob->state.load(std::memory_order_acquire) < 0 && opt_.specializeStrict)

@@ -182,6 +182,7 @@ struct EngineOptions {
                                   // with the number of resident warps, so the gain is far from the stage count (DESIGN.md section 4)
     int specMinBlocks = 0;        // > 0: specialised kernels of the narrow geometries (1 < L < 32) are compiled for this many CTAs per SM (8 = 64 registers)
     bool specializeStrict = false; // a failed specialisation is an error (COMMIT returns 7 / process -1) instead of a silent stay on the interpreter
+    bool specOpprof = false;      // specialised kernels carry the per-opcode cycle counters (-DEB_OPPROF; tools/spec_opprof.py); profiling only
 };
 
 class Engine {
@@ -270,6 +271,8 @@ public:
     // Compile (not load, not run) the specialised K1 of the voice group containing `voice`: returns the cubin size or -1, the
     // NVRTC log in `log`.  Works without a GPU (NVRTC is a pure compiler): the CPU test-suite uses it.
     long specializeDryRun(int voice, std::string& log);
+    // Adds the per-opcode counters of the loaded specialised kernels compiled with option spec_opprof (each kernel once) to out128.
+    bool specOpprofRead(unsigned long long* out128, bool reset);
 
 private:
     // Threading contract of the boundary (Runtime.h:133,204,277-285: one control thread + one render thread, concurrently): every

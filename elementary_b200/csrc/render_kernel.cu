@@ -105,6 +105,19 @@ __device__ __forceinline__ double clampd(double v, double lo, double hi) { retur
 __device__ __forceinline__ float stdmin(float a, float b) { return (b < a) ? b : a; }   // std::min
 __device__ __forceinline__ float stdmax(float a, float b) { return (a < b) ? b : a; }   // std::max
 
+// OP_DELAY's hoisted read window (render_ops.inc): true when readFrac = (float) (size + w) - offset is exact for every w in
+// [0, size), so that readLeft = size + w - ceil(offset) and frac = ceil(offset) - offset for every sample.  offset's lowest set
+// bit is worth 2^-f (f fractional bits, 0 for an integer); every size + w - offset is a multiple of 2^-f below 2 size and fits
+// the 24-bit significand when 2 size <= 2^(24 - f) (which also keeps (float) (size + w) exact).  For offset >= 1, the fast
+// path's hazard bound (tests/test_delay_window_cpu.py sweeps it against the float computation).
+__device__ __forceinline__ bool delay_offset_exact(float offset, int size) {
+    const uint32_t b = __float_as_uint(offset);
+    const int e = (int) (b >> 23) - 127;                 // unbiased exponent (offset positive and normal)
+    const int tz = __ffs((int) (b | 0x800000u)) - 1;     // trailing zero bits of the significand, implicit bit included
+    const int f = max(0, 23 - e - tz);
+    return f <= 23 && ((size - 1) >> (23 - f)) == 0;
+}
+
 // helpers/Change.h:12-32
 __device__ __forceinline__ float change_tick(float& lastIn, float xn) {
     const float dt = xn - lastIn;
@@ -655,7 +668,14 @@ __device__ __forceinline__ void render_tile(const LaunchParams& P, const int til
 #define CHAIN_NEXT(s) ((void) 0)
 #define PC_ADVANCE(n) ((void) 0)
 #define PC_SKIP_SEGMENT_IF(cond, n) ((void) 0)
+#ifdef EB_OPPROF
+                            const long long prof_t0 = clock64();
+#endif
 #include "render_ops.inc"
+#ifdef EB_OPPROF
+                            __syncwarp();
+                            if (lane == 0) { atomicAdd(&g_opprof[2 * (opcode & 63)], (unsigned long long) (clock64() - prof_t0)); atomicAdd(&g_opprof[2 * (opcode & 63) + 1], 1ull); }
+#endif
 #undef CHAIN_NEXT
 #undef OPWORD
 #undef CHAIN_FOR_STEPS

@@ -47,6 +47,7 @@ struct Api {
     decltype(&cuFuncGetAttribute) funcGetAttribute = nullptr;
     decltype(&cuLaunchKernel) launchKernel = nullptr;
     decltype(&cuGetErrorString) getErrorString = nullptr;
+    decltype(&cuModuleGetGlobal) moduleGetGlobal = nullptr;   // optional: only opprof kernels use it
 };
 
 template <typename F>
@@ -98,6 +99,7 @@ bool loadDriver(std::string& log) {
                      sym(h, "cuFuncGetAttribute", a.funcGetAttribute) && sym(h, "cuLaunchKernel", a.launchKernel) &&
                      sym(h, "cuGetErrorString", a.getErrorString);
         if (!a.driverOk) { a.driverErr = "libcuda lacks a required entry point"; dlclose(h); }
+        else sym(h, "cuModuleGetGlobal_v2", a.moduleGetGlobal);
     });
     if (!a.driverOk) log = a.driverErr;
     return a.driverOk;
@@ -137,7 +139,7 @@ void workerLoop(std::shared_ptr<Queue> q) {
             q->busy = true;
         }
         std::string log;
-        const bool ok = specialise_compile(job->code, job->tileWidth, job->niterOverride, job->customSource, job->kernel, log, job->minBlocks);
+        const bool ok = specialise_compile(job->code, job->tileWidth, job->niterOverride, job->customSource, job->kernel, log, job->minBlocks, job->opprof);
         {
             std::lock_guard<std::mutex> lk(q->m);
             job->log = log;
@@ -175,7 +177,7 @@ std::vector<uint32_t> specialise_key_words(const std::vector<uint32_t>& code) {
 }
 
 bool specialise_compile(const std::vector<uint32_t>& codeIn, int tileWidth, int niterOverride, const std::string& customSource, SpecKernel& out, std::string& log,
-                        int minBlocks) {
+                        int minBlocks, bool opprof) {
     if (!loadNvrtc(log)) return false;
     Api& a = api();
     const std::vector<uint32_t> code = specialise_key_words(codeIn);
@@ -197,10 +199,13 @@ bool specialise_compile(const std::vector<uint32_t>& codeIn, int tileWidth, int 
     const int niter = render_niter_for(tileWidth, niterOverride);
     const std::string name = "eb::render_block_kernel<" + std::to_string(niter) + ", " + std::to_string(logl) + ">";
     a.addNameExpression(prog, name.c_str());
+    const char* const opprofExpr = "&eb::g_opprof";
+    if (opprof) a.addNameExpression(prog, opprofExpr);
     const std::string mb = "-DEB_NARROW_MINBLOCKS=" + std::to_string(minBlocks > 0 ? minBlocks : 4);
     const char* opts[] = {"--std=c++20", "--gpu-architecture=sm_90a", "--fmad=false", "-lineinfo", "-default-device",
-                          "--pre-include=eb_spec_program.h", "-diag-suppress=186,68,179,177", mb.c_str()};
-    const nvrtcResult rc = a.compileProgram(prog, (int) (sizeof(opts) / sizeof(opts[0])), opts);
+                          "--pre-include=eb_spec_program.h", "-diag-suppress=186,68,179,177", mb.c_str(), "-DEB_OPPROF"};
+    const int nOpts = (int) (sizeof(opts) / sizeof(opts[0])) - (opprof ? 0 : 1);
+    const nvrtcResult rc = a.compileProgram(prog, nOpts, opts);
     size_t n = 0;
     a.getLogSize(prog, &n);
     if (n > 1) { log.resize(n); a.getLog(prog, &log[0]); }
@@ -212,6 +217,8 @@ bool specialise_compile(const std::vector<uint32_t>& codeIn, int tileWidth, int 
         if (ok) { out.cubin.resize(sz); ok = a.getCubin(prog, out.cubin.data()) == NVRTC_SUCCESS; }
         const char* ln = nullptr;
         if (ok && a.getLoweredName(prog, name.c_str(), &ln) == NVRTC_SUCCESS && ln) lowered = ln; else ok = false;
+        const char* pn = nullptr;
+        if (ok && opprof) { if (a.getLoweredName(prog, opprofExpr, &pn) == NVRTC_SUCCESS && pn) out.opprofName = pn; else ok = false; }
     }
     a.destroyProgram(&prog);
     if (!ok) { if (log.empty()) log = "NVRTC compilation failed"; return false; }
@@ -232,13 +239,20 @@ bool specialise_load(SpecKernel& k, std::string& log) {
     if (r != CUDA_SUCCESS) { a.moduleUnload(mod); log = "cuModuleGetFunction failed for " + k.loweredName + ": " + cuErr(r); return false; }
     a.funcGetAttribute(&k.numRegs, CU_FUNC_ATTRIBUTE_NUM_REGS, fn);
     a.funcGetAttribute(&k.localBytes, CU_FUNC_ATTRIBUTE_LOCAL_SIZE_BYTES, fn);
+    if (!k.opprofName.empty()) {
+        CUdeviceptr p = 0;
+        size_t bytes = 0;
+        r = a.moduleGetGlobal ? a.moduleGetGlobal(&p, &bytes, mod, k.opprofName.c_str()) : CUDA_ERROR_NOT_FOUND;
+        if (r != CUDA_SUCCESS) { a.moduleUnload(mod); log = "cuModuleGetGlobal failed for the opprof counters: " + cuErr(r); return false; }
+        k.opprofPtr = (unsigned long long) p;
+    }
     k.module = mod;
     k.function = fn;
     return true;
 }
 
 std::shared_ptr<SpecJob> specialise_request(const std::vector<uint32_t>& code, int tileWidth, int niterOverride, int device, const std::string& customSource,
-                                            int minBlocks) {
+                                            int minBlocks, bool opprof) {
     // Load NVRTC (and so register waitForCompilerAtExit) on THIS thread, before any job can reach the worker: loaded lazily by the
     // worker, a process that queues a job and exits at once could start exiting before the handler exists, and the worker would then
     // run NVRTC while its statics are torn down.  A load failure is reported by the job itself.
@@ -249,7 +263,7 @@ std::shared_ptr<SpecJob> specialise_request(const std::vector<uint32_t>& code, i
     auto q = queue();
     const std::vector<uint32_t> key = specialise_key_words(code);
     std::string k(reinterpret_cast<const char*>(key.data()), key.size() * sizeof(uint32_t));
-    k += "|c" + customSource + "|L" + std::to_string(tileWidth) + "|n" + std::to_string(render_niter_for(tileWidth, niterOverride)) + "|d" + std::to_string(device) + "|b" + std::to_string(minBlocks);
+    k += "|c" + customSource + "|L" + std::to_string(tileWidth) + "|n" + std::to_string(render_niter_for(tileWidth, niterOverride)) + "|d" + std::to_string(device) + "|b" + std::to_string(minBlocks) + "|p" + (opprof ? "1" : "0");
     std::lock_guard<std::mutex> lk(q->m);
     auto it = q->cache.find(k);
     if (it != q->cache.end() && it->second->state.load(std::memory_order_acquire) >= 0) return it->second;
@@ -259,6 +273,7 @@ std::shared_ptr<SpecJob> specialise_request(const std::vector<uint32_t>& code, i
     job->tileWidth = tileWidth;
     job->niterOverride = niterOverride;
     job->minBlocks = minBlocks;
+    job->opprof = opprof;
     q->cache[k] = job;
     q->jobs.push_back(job);
     if (!q->workerStarted) {
@@ -286,6 +301,15 @@ int specialise_ensure_loaded(SpecJob& job) {
     if (!ok) job.log = log;
     job.state.store(ok ? 2 : -1, std::memory_order_release);
     return ok ? 2 : -1;
+}
+
+bool specialise_opprof_read(const SpecKernel& k, unsigned long long* out128, bool reset) {
+    if (!k.opprofPtr) return true;
+    unsigned long long buf[128];
+    void* dev = reinterpret_cast<void*>((uintptr_t) k.opprofPtr);   // unified addressing: the module's global as a runtime-API pointer
+    if (cudaMemcpy(buf, dev, sizeof buf, cudaMemcpyDeviceToHost) != cudaSuccess) return false;
+    for (int i = 0; i < 128; ++i) out128[i] += buf[i];
+    return !reset || cudaMemset(dev, 0, sizeof buf) == cudaSuccess;
 }
 
 cudaError_t specialise_launch(const SpecKernel& k, const LaunchParams& P, int grid, int threads, size_t smem, int perWarpFloats, cudaStream_t stream) {

@@ -31,12 +31,16 @@ struct SpecKernel {
     std::vector<char> cubin;
     std::string loweredName;     // mangled name of the kernel inside the cubin
     int numRegs = 0, localBytes = 0;   // filled by specialise_load (cuFuncGetAttribute): reported by describe()
+    std::string opprofName;      // -DEB_OPPROF builds: mangled name of the per-opcode counter array g_opprof
+    unsigned long long opprofPtr = 0;  // its device address once loaded
 };
 
 // Step 1 — pure compilation (NVRTC only; thread safe, needs no CUDA context, works without a GPU): K1 for (tileWidth,
 // niterOverride) against `code` (one single-stage program).  Fills out.cubin / out.loweredName.
+// minBlocks > 0: CTAs per SM the narrow geometries (1 < L < 32) are compiled for (8 = 64 registers); opprof: compile the per-opcode
+// cycle counters in (-DEB_OPPROF, read with specialise_opprof_read).
 bool specialise_compile(const std::vector<uint32_t>& code, int tileWidth, int niterOverride, const std::string& customSource, SpecKernel& out, std::string& log,
-                        int minBlocks = 0);   // minBlocks > 0: CTAs per SM the narrow geometries (1 < L < 32) are compiled for (8 = 64 registers)
+                        int minBlocks = 0, bool opprof = false);
 // Step 2 — on a thread whose CUDA context is current: load the cubin and resolve the kernel (milliseconds).
 bool specialise_load(SpecKernel& k, std::string& log);
 
@@ -49,11 +53,15 @@ struct SpecJob {
     std::vector<uint32_t> code;
     std::string customSource;
     int tileWidth = 0, niterOverride = 0, minBlocks = 0;
+    bool opprof = false;
 };
 // Queue (or find in the cache) the specialisation of `code` for a tile geometry on `device`.  Never blocks on the compiler.
 // customSource: device text of the registered node types the program may use (Engine::customSource; empty = none) — compiled in front of the kernel.
 std::shared_ptr<SpecJob> specialise_request(const std::vector<uint32_t>& code, int tileWidth, int niterOverride, int device, const std::string& customSource,
-                                            int minBlocks = 0);
+                                            int minBlocks = 0, bool opprof = false);
+// A loaded kernel compiled with opprof: adds its counters (out128[2 * op] cycles, [2 * op + 1] dispatches, op 63 = whole sample loop of a
+// warp) to out128, optionally zeroing them.  A kernel without counters adds nothing.
+bool specialise_opprof_read(const SpecKernel& k, unsigned long long* out128, bool reset);
 // Block until the job has left state 0 (used by option "specialize" = 2 and by tests).
 void specialise_wait(SpecJob& job);
 // Render thread: load a compiled job (state 1 -> 2 / -1).  Returns the state afterwards.

@@ -209,7 +209,8 @@ int elem_b200_program_words(elem_b200_runtime* rt, int voice, uint32_t* buf, siz
  * containing `voice` (no GPU needed) and returns the cubin size, or -1 with the compiler log in logBuf. */
 long elem_b200_specialize_dry_run(elem_b200_runtime* rt, int voice, char* logBuf, size_t cap);
 /* A/B builds of the library compiled with -DEB_OPPROF (tools/opprof.py) only: cycles (out128[2*op]) and dispatch counts
- * (out128[2*op+1]) per opcode of the K1 interpreter since the last reset; the product library writes zeros.  No reference counterpart:
+ * (out128[2*op+1]) per opcode of the K1 interpreter since the last reset; the product library writes zeros.  Engine option
+ * "spec_opprof" = 1 compiles the same counters into the specialised kernels (any library build); theirs are added in.  No reference counterpart:
  * this is what the pipeline cost model of the host compiler is calibrated against.  Returns 0, or -1 on a CUDA error. */
 int elem_b200_debug_opprof(elem_b200_runtime* rt, unsigned long long* out128, int reset);
 /* Number of CUDA kernels this runtime has launched so far. */
