@@ -2165,7 +2165,7 @@ int Engine::compile(Group& g, int nIn, std::shared_ptr<Program>& out) {
             prog->code.push_back(make_w0(op.opcode, (uint32_t) nOperandWords, (uint32_t) slot, op.mode));
             prog->code.push_back(st);
             prog->code.push_back(op.aux0);
-            prog->code.push_back(op.aux1);
+            prog->code.push_back(op.opcode == OP_DELAY ? (uint32_t) ++prog->nDelayBuf : op.aux1);   // OP_DELAY: 1 + its read-window buffer
             prog->code.push_back((uint32_t) op.ptr);
             prog->code.push_back((uint32_t) (op.ptr >> 32));
             prog->code.push_back((uint32_t) (op.opcode == OP_CHAIN ? op.steps.size() : op.operands.size()));
@@ -2571,7 +2571,8 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
         // launch geometry: spread warps over the SMs first, then stack them
         int wpc = opt_.warpsPerCta;
         if (wpc <= 0) wpc = nTiles >= smCount_ * 8 ? 4 : (nTiles >= smCount_ * 4 ? 2 : 1);
-        const size_t perWarp = render_smem_bytes(p.nSlots, P.nOut, p.nStateRows, (int) p.paramMap.size(), 1, g.tileWidth, opt_.niter);
+        const size_t perWarp = render_smem_bytes(p.nSlots, P.nOut, p.nStateRows, (int) p.paramMap.size(), 1, g.tileWidth, opt_.niter) +
+                               render_delay_buf_floats(p.nDelayBuf, g.tileWidth, opt_.niter) * sizeof(float);
         while (wpc > 1 && perWarp * wpc > 200 * 1024) wpc >>= 1;
         if (perWarp > 220 * 1024) return fail(rc::InvariantViolation, "graph state does not fit in shared memory");
         const size_t nStages = std::max<size_t>(1, p.stages.size());
@@ -2604,6 +2605,7 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
                     if (st == 2) spec = &p.specJob->kernel;
                     else if (st < 0 && (opt_.specializeStrict || p.hasCustom)) return fail(rc::CudaError, "K1 specialisation failed: " + p.specJob->log);
                 }
+                P.nDelayBuf = p.nDelayBuf;      // (the many-groups launches above reserve no read-window buffers: 0)
                 if (!dry && !cuda(launch_render_block(P, wpc, opt_.niter, stream_, spec), "render kernel launch")) return rc::CudaError;
                 ++launches_;
             }

@@ -120,6 +120,7 @@ struct Program {
     int nOps = 0;
     int nStateRows = 0;
     int nSlots = 1;
+    int nDelayBuf = 0;           // OP_DELAY ops (aux1 = 1 + the index of the op's read-window buffer, LaunchParams::nDelayBuf)
     int nIn = 0;
     bool usesHostInputs = false;
     std::vector<int32_t> rootIds;         // root index -> node id

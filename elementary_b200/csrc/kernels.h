@@ -9,6 +9,7 @@ namespace eb {
 // K1: fused render-sequence kernel, one launch per voice group per block.
 int render_niter_for(int tileWidth, int niterOverride);   // elements per lane per sample tile (E = 32*NITER = L*T)
 size_t render_smem_bytes(int nSlots, int nOut, int nStateRows, int nParams, int warpsPerCta, int tileWidth, int niterOverride);
+int render_delay_buf_floats(int nDelayBuf, int tileWidth, int niterOverride);   // per warp, a multiple of 4
 struct SpecKernel;   // spec_host.h: K1 compiled at run time against one program (nullptr = the built-in interpreter)
 cudaError_t launch_render_block(const LaunchParams& P, int warpsPerCta, int niterOverride, cudaStream_t stream, const SpecKernel* spec = nullptr);
 

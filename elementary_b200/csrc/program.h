@@ -151,6 +151,8 @@ struct LaunchParams {
     const float* tableSrc;       // device copy of the resource (16-byte aligned, padded to a multiple of 16 bytes), or null
     int tableFloats;             // padded length in floats
     int tableSmem;               // float index of the staged copy in the CTA's dynamic shared memory, or -1
+    int nDelayBuf;               // read-window buffers of OP_DELAY, [nDelayBuf][T + 1][L] floats behind each warp's parameter rows
+                                 // (single-group launches: render_delay_buf_floats; 0 = none, every delay loads its window itself)
     // Stage pipeline (render_groups_pipe_kernel; one-voice groups, BASELINE config 5): the host cut the program into pipeW contiguous
     // stages; pipeW warps of ONE CTA share the graph's shared-memory area, warp w runs stage w, one sample tile behind warp w - 1.
     // Values crossing a stage boundary live in ring slots (pipeDepth buffers, buffer = tile index mod pipeDepth).  0 / 1 = not pipelined.

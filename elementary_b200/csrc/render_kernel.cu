@@ -573,32 +573,67 @@ __device__ __forceinline__ void render_tile(const LaunchParams& P, const int til
         return o;
     };
 
-    // ---- state and parameter rows HBM -> shared memory (once per block), by the owner lanes ----
+#ifdef EB_OPPROF
+    const long long prof_entry = clock64();
+#endif
+    // ---- state and parameter rows HBM -> shared memory (once per block) ----
     // (a pipeline stage stages the state rows of ITS ops only; stage 0 also stages the parameters — the later stages read them after
     // their first hand-over from the stage before, which orders them behind these stores)
+    constexpr int SPASS = 32 >> LOGL;     // state entries (and parameters) per pass of the lane-parallel form
     const int stateBegin = (PIPE && pipeW > 1) ? (int) P.pipeState[stage] : 0;
     const int stateEnd = (PIPE && pipeW > 1) ? (int) P.pipeState[stage + 1] : P.nStateEntries;
     const int srowBegin = (PIPE && pipeW > 1) ? (int) P.pipeSrow[stage] : 0;
-    if (owner) {
-        int srow = srowBegin;
-        for (int i = stateBegin; i < stateEnd; ++i) {
-            const uint32_t m = __ldg(P.stateMap + i);
-            if (m == STATE_PAD) { srow += 1; continue; }
-            const size_t row = m & ~STATE_DOUBLE_FLAG;
-            if (m & STATE_DOUBLE_FLAG) {
-                const double* g = reinterpret_cast<const double*>(P.rows + row * P.Vpad);
-                reinterpret_cast<double*>((sst + srow * L).ptr())[lane] = g[voice];
-                srow += 2;
-            } else {
-                sst[srow * L + lane] = P.rows[row * P.Vpad + voice];
-                srow += 1;
+    auto state_row = [&](uint32_t dmask, int srow) { return srow + tlane + (__popc(dmask & ((1u << (tlane << LOGL)) - 1u)) >> LOGL); };
+    if constexpr (PIPE) {
+        // The pipelined one-voice interpreter (BASELINE config 5) keeps the owner lane's serial loop: the lane-parallel form below made
+        // that kernel 1.5 % slower on an H100 (DESIGN.md section 4).
+        if (owner) {
+            int srow = srowBegin;
+            for (int i = stateBegin; i < stateEnd; ++i) {
+                const uint32_t m = __ldg(P.stateMap + i);
+                if (m == STATE_PAD) { srow += 1; continue; }
+                const size_t row = m & ~STATE_DOUBLE_FLAG;
+                if (m & STATE_DOUBLE_FLAG) {
+                    const double* g = reinterpret_cast<const double*>(P.rows + row * P.Vpad);
+                    reinterpret_cast<double*>((sst + srow * L).ptr())[lane] = g[voice];
+                    srow += 2;
+                } else {
+                    sst[srow * L + lane] = P.rows[row * P.Vpad + voice];
+                    srow += 1;
+                }
+            }
+            if (firstStage) {
+                spar[lane] = 0.0f;
+                for (int i = 0; i < P.nParams; ++i)
+                    spar[(i + 1) * L + lane] = __ldg(P.rows + (size_t) __ldg(P.paramMap + i) * P.Vpad + voice);
             }
         }
-        if (firstStage) {
-            spar[lane] = 0.0f;
-            for (int i = 0; i < P.nParams; ++i)
-                spar[(i + 1) * L + lane] = __ldg(P.rows + (size_t) __ldg(P.paramMap + i) * P.Vpad + voice);
+    } else {
+        // Every warp of the grid is here at the same moment, so nothing hides these loads: all 32 lanes take part.  Lane `lane` stages
+        // state entry pass * SPASS + tlane and parameter pass * SPASS + tlane for voice `vlane`, and a pass issues all of its row loads
+        // before its first shared-memory store — one dependent map -> row round trip per pass instead of one per entry.  An entry's
+        // shared-memory row is the pass's first row + its index in the pass + the doubles before it (one extra row each), by warp vote.
+        const int nParams = P.nParams;
+        int srow = srowBegin;
+        for (int i0 = stateBegin, j0 = 0; i0 < stateEnd || j0 < nParams; i0 += SPASS, j0 += SPASS) {
+            const int i = i0 + tlane, j = j0 + tlane;
+            const uint32_t m = (i < stateEnd) ? __ldg(P.stateMap + i) : STATE_PAD;
+            const uint32_t pm = (j < nParams) ? __ldg(P.paramMap + j) : 0u;
+            const bool dbl = m != STATE_PAD && (m & STATE_DOUBLE_FLAG);
+            const size_t row = m & ~STATE_DOUBLE_FLAG;
+            double d = 0.0;
+            float f = 0.0f, pv = 0.0f;
+            if (dbl) d = reinterpret_cast<const double*>(P.rows + row * P.Vpad)[voice];
+            else if (m != STATE_PAD) f = P.rows[row * P.Vpad + voice];
+            if (j < nParams) pv = __ldg(P.rows + (size_t) pm * P.Vpad + voice);
+            const uint32_t dmask = __ballot_sync(FULL, dbl);
+            const int r = state_row(dmask, srow);
+            if (dbl) reinterpret_cast<double*>((sst + r * L).ptr())[vlane] = d;
+            else if (m != STATE_PAD) sst[r * L + vlane] = f;
+            if (j < nParams) spar[(j + 1) * L + vlane] = pv;
+            srow += SPASS + (__popc(dmask) >> LOGL);
         }
+        if (owner) spar[lane] = 0.0f;
     }
     __syncwarp();
 
@@ -832,23 +867,49 @@ __device__ __forceinline__ void render_tile(const LaunchParams& P, const int til
 #ifdef EB_OPPROF
     if (lane == 0) { atomicAdd(&g_opprof[2 * 63], (unsigned long long) (clock64() - prof_tile0)); atomicAdd(&g_opprof[2 * 63 + 1], 1ull); }   // whole sample loop of one warp
 #endif
-    // ---- state rows shared memory -> HBM ----
-    if (owner) {
-        int srow = srowBegin;
-        for (int i = stateBegin; i < stateEnd; ++i) {
-            const uint32_t m = __ldg(P.stateMap + i);
-            if (m == STATE_PAD) { srow += 1; continue; }
-            const size_t row = m & ~STATE_DOUBLE_FLAG;
-            if (m & STATE_DOUBLE_FLAG) {
-                double* g = reinterpret_cast<double*>(P.rows + row * P.Vpad);
-                g[voice] = reinterpret_cast<const double*>((sst + srow * L).ptr())[lane];
-                srow += 2;
-            } else {
-                P.rows[row * P.Vpad + voice] = sst[srow * L + lane];
-                srow += 1;
+#ifdef EB_OPPROF
+    const long long prof_wb0 = clock64();
+#endif
+    // ---- state rows shared memory -> HBM, in the form of the staging prologue ----
+    if constexpr (PIPE) {
+        if (owner) {
+            int srow = srowBegin;
+            for (int i = stateBegin; i < stateEnd; ++i) {
+                const uint32_t m = __ldg(P.stateMap + i);
+                if (m == STATE_PAD) { srow += 1; continue; }
+                const size_t row = m & ~STATE_DOUBLE_FLAG;
+                if (m & STATE_DOUBLE_FLAG) {
+                    double* g = reinterpret_cast<double*>(P.rows + row * P.Vpad);
+                    g[voice] = reinterpret_cast<const double*>((sst + srow * L).ptr())[lane];
+                    srow += 2;
+                } else {
+                    P.rows[row * P.Vpad + voice] = sst[srow * L + lane];
+                    srow += 1;
+                }
             }
         }
+    } else {
+        int srow = srowBegin;
+        for (int i0 = stateBegin; i0 < stateEnd; i0 += SPASS) {
+            const int i = i0 + tlane;
+            const uint32_t m = (i < stateEnd) ? __ldg(P.stateMap + i) : STATE_PAD;
+            const bool dbl = m != STATE_PAD && (m & STATE_DOUBLE_FLAG);
+            const size_t row = m & ~STATE_DOUBLE_FLAG;
+            const uint32_t dmask = __ballot_sync(FULL, dbl);
+            const int r = state_row(dmask, srow);
+            if (dbl) reinterpret_cast<double*>(P.rows + row * P.Vpad)[voice] = reinterpret_cast<const double*>((sst + r * L).ptr())[vlane];
+            else if (m != STATE_PAD) P.rows[row * P.Vpad + voice] = sst[r * L + vlane];
+            srow += SPASS + (__popc(dmask) >> LOGL);
+        }
     }
+#ifdef EB_OPPROF
+    __syncwarp();
+    if (lane == 0) {   // staging prologue (entry to the first tile) and state write-back of one warp
+        const long long prof_wb1 = clock64();
+        atomicAdd(&g_opprof[2 * 61], (unsigned long long) (prof_tile0 - prof_entry)); atomicAdd(&g_opprof[2 * 61 + 1], 1ull);
+        atomicAdd(&g_opprof[2 * 62], (unsigned long long) (prof_wb1 - prof_wb0)); atomicAdd(&g_opprof[2 * 62 + 1], 1ull);
+    }
+#endif
 
     // ---- tap promotion (GraphRenderSequence.h:200-210,306-308): OP_PROMOTE records after the first OP_END ----
     if (!(PIPE && pipeW > 1)) {    // (the host never pipelines a program with taps)
@@ -1032,6 +1093,11 @@ int render_niter_for(int tileWidth, int niterOverride) {
     return tileWidth == 2 ? 4 : 1;   // L = 1 keeps T = 32: with one voice per warp longer tiles push delay lines off their fast path (config 5)
 }
 
+int render_delay_buf_floats(int nDelayBuf, int tileWidth, int niterOverride) {
+    const int T = 32 * render_niter_for(tileWidth, niterOverride) / tileWidth;
+    return (nDelayBuf * (T + 1) * tileWidth + 3) & ~3;
+}
+
 size_t render_smem_bytes(int nSlots, int nOut, int nStateRows, int nParams, int warpsPerCta, int tileWidth, int niterOverride) {
     const int E = 32 * render_niter_for(tileWidth, niterOverride);
     const size_t perWarp = ((size_t) (nSlots + nOut) * E + (size_t) (nStateRows + nParams + 1) * tileWidth + 3) & ~(size_t) 3;
@@ -1066,7 +1132,9 @@ cudaError_t launch_render_block(const LaunchParams& P, int warpsPerCta, int nite
     if (nTiles <= 0) return cudaSuccess;
     const int grid = (nTiles + warpsPerCta - 1) / warpsPerCta;
     const int threads = warpsPerCta * 32;
-    size_t smem = render_smem_bytes(P.nSlots, P.nOut, P.nStateRows, P.nParams, warpsPerCta, L, niterOverride);
+    // + the delays' read-window buffers behind each warp's parameter rows (render_ops.inc OP_DELAY)
+    size_t smem = render_smem_bytes(P.nSlots, P.nOut, P.nStateRows, P.nParams, warpsPerCta, L, niterOverride) +
+                  (size_t) warpsPerCta * render_delay_buf_floats(P.nDelayBuf, L, niterOverride) * sizeof(float);
     LaunchParams Q = P;
     const int perWarpFloats = (int) (smem / sizeof(float) / warpsPerCta);
     if (Q.tableSrc && Q.tableFloats > 0 && Q.tableFloats <= TABLE_SMEM_MAX_FLOATS &&
