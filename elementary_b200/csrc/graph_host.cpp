@@ -210,7 +210,8 @@ Engine::~Engine() {
     if (dInShared_) dfree(dInShared_);
     if (hPinned_ && !planOnly_) cudaFreeHost(hPinned_);
     if (hMixHost_) cudaFreeHost(hMixHost_);
-    for (int i = 0; i < 2; ++i) { if (offlineDev_[i]) cudaFree(offlineDev_[i]); if (offlinePinned_[i]) cudaFreeHost(offlinePinned_[i]); }
+    for (OfflineBuf* b : {&offOut_, &offIn_, &offMix_})
+        for (int i = 0; i < 2; ++i) { if (b->dev[i]) cudaFree(b->dev[i]); if (b->pinned[i]) cudaFreeHost(b->pinned[i]); }
     if (dDeliverDone_) cudaFree(dDeliverDone_);
     if (wide_.dRows) dfree(wide_.dRows);
     if (wide_.dSegs) dfree(wide_.dSegs);
@@ -2320,6 +2321,7 @@ int Engine::ensureBuffers(size_t nIn, size_t nOut, bool perVoiceIn, bool materia
             } else { hMixHost_ = nullptr; cudaGetLastError(); }
         }
     }
+    if (offlineIn_) return rc::Ok;   // the inputs are in an offline chunk
     if (perVoiceIn && nIn) { if (!voiceInDevicePtr(nIn)) return rc::CudaError; }
     else if (nIn) { if (!sharedInDevicePtr(nIn)) return rc::CudaError; }
     return rc::Ok;
@@ -2368,14 +2370,21 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
     if (wide && offlineOut_) return fail(rc::BadArgument, "renderOffline: at most 8 output channels");
     if (!wide && materialise && !offlineOut_) wide_.outZeroValid = false;   // K1 writes [voice][nOut] in the dense layout
 
-    const size_t key[6] = {nIn, nOut, numSamples, (size_t) perVoiceIn, (size_t) materialise | ((size_t) (uintptr_t) offlineOut_ << 1), (size_t) mix | ((size_t) offlineStride_ << 1)};
+    // the cached descriptors hold the I/O base pointers: any change of where inputs or outputs live (an offline chunk slot) is a new key
+    const size_t key[7] = {nIn, nOut, numSamples, (size_t) perVoiceIn, (size_t) materialise | ((size_t) (uintptr_t) offlineOut_ << 1),
+                           (size_t) mix | ((size_t) offlineStride_ << 1), (size_t) (uintptr_t) offlineIn_};
+    // an offline block reads its inputs from column offlineOffset_ of the input chunk and leaves its mix in the same column of the mix chunk
+    const int inStride = offlineIn_ ? offlineStride_ : blockSize_, inOffset = offlineIn_ ? offlineOffset_ : 0;
+    const int outOffset = offlineOut_ ? offlineOffset_ : 0;
+    float* const mixDst = offlineMix_ ? offlineMix_ + offlineOffset_ : dMix_;
+    const int mixStride = offlineMix_ ? offlineStride_ : blockSize_;
     if (steadyValid_ && !dry && std::memcmp(key, steadyKey_, sizeof key) == 0) {
         for (auto& sb : steadyBuckets_) {
             BatchBuffers& bb = batch_[sb.key];
             auto ev = timedBegin();
             if (!cuda(sb.pipeStages >= 1
-                          ? launch_render_groups_pipe(bb.dDescs, bb.dTileStart, sb.nGroups, sb.totalTiles, sb.pipeStages, sb.maxSlots, sb.smemOut, sb.maxState, sb.maxParams, sampleTime_, offlineOut_ ? offlineOffset_ : 0, stream_, opt_.niter)
-                          : launch_render_groups(bb.dDescs, bb.dTileStart, sb.nGroups, sb.totalTiles, sb.L, sb.maxSlots, sb.smemOut, sb.maxState, sb.maxParams, sb.wpc, sampleTime_, offlineOut_ ? offlineOffset_ : 0, stream_, opt_.niter),
+                          ? launch_render_groups_pipe(bb.dDescs, bb.dTileStart, sb.nGroups, sb.totalTiles, sb.pipeStages, sb.maxSlots, sb.smemOut, sb.maxState, sb.maxParams, sampleTime_, outOffset, inOffset, stream_, opt_.niter)
+                          : launch_render_groups(bb.dDescs, bb.dTileStart, sb.nGroups, sb.totalTiles, sb.L, sb.maxSlots, sb.smemOut, sb.maxState, sb.maxParams, sb.wpc, sampleTime_, outOffset, inOffset, stream_, opt_.niter),
                       "render groups kernel launch")) return rc::CudaError;
             if (timeKernels_) { cudaEventRecord(ev.second, stream_); timedEvents_.push_back(ev); }
             ++launches_;
@@ -2385,7 +2394,7 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
             if (rw != rc::Ok) return rw;
         } else if (mix) {
             auto ev = timedBegin();
-            if (!cuda(launch_mix_reduce(dPartial_, dMix_, dMixScratch_, dMixTickets_, steadyTiles_, (int) nOut, blockSize_, (int) numSamples, stream_, takeDeliver()), "mix reduce launch")) return rc::CudaError;
+            if (!cuda(launch_mix_reduce(dPartial_, mixDst, mixStride, dMixScratch_, dMixTickets_, steadyTiles_, (int) nOut, blockSize_, (int) numSamples, stream_, takeDeliver()), "mix reduce launch")) return rc::CudaError;
             if (timeKernels_) { cudaEventRecord(ev.second, stream_); timedMixEvents_.push_back(ev); }
             ++launches_;
         }
@@ -2469,6 +2478,7 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
     }
     int r = ensureBuffers(nIn, nOut, perVoiceIn, materialise, wideRows, wideOutRows);
     if (r != rc::Ok) return r;
+    const float* const inBase = offlineIn_ ? offlineIn_ : (perVoiceIn ? dInVoice_ : dInShared_);   // (ensureBuffers may have moved these)
     if (wide && !dry) {
         r = uploadWidePlan();
         if (r != rc::Ok) return r;
@@ -2496,13 +2506,16 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
         P.paramMap = p.dParamMap;
         P.nParams = (int) p.paramMap.size();
         P.rows = g.dRows;
-        P.inShared = (!perVoiceIn && nIn) ? dInShared_ : nullptr;
-        P.inVoice = (perVoiceIn && nIn) ? dInVoice_ : nullptr;
         // wide: the group's own runs of compact rows, per-voice I/O indexed from its first voice (voice0 = 0)
         const std::vector<int>* const gch = wide ? &wideCh[gi] : nullptr;
         float* const voiceOut = wide ? (gch->empty() ? nullptr : dOutCompact_ + wideOutBase[gi] * blockSize_) : (offlineOut_ ? offlineOut_ : dOutVoice_);
         float* const partialOut = wide ? (gch->empty() ? nullptr : dPartial_ + wideRowBase[gi] * blockSize_) : dPartial_;
-        if (wide && P.inVoice) P.inVoice += (size_t) g.v0 * nIn * blockSize_;
+        // input rows without this block's column offset (the many-groups launches take it as an argument; single-group launches are
+        // handed pointers that include it)
+        const float* const inShared = (!perVoiceIn && nIn) ? inBase : nullptr;
+        const float* const inVoice = (perVoiceIn && nIn) ? inBase + (wide ? (size_t) g.v0 * nIn * inStride : 0) : nullptr;
+        P.inShared = inShared;
+        P.inVoice = inVoice;
         P.outVoice = materialise ? voiceOut : nullptr;
         P.mixPartial = mix ? partialOut : nullptr;
         P.nStateEntries = (int) p.stateMap.size();
@@ -2516,7 +2529,7 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
         P.blockSize = blockSize_;
         P.nIn = (int) nIn;
         P.nOut = wide ? (int) gch->size() : (int) nOut;
-        P.inStride = blockSize_;
+        P.inStride = inStride;
         P.outStride = offlineOut_ ? offlineStride_ : blockSize_;
         P.tileBase = wide ? 0 : tileBase;
         uint32_t runMask = 0;
@@ -2589,7 +2602,9 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
             allBatched = false;
             const bool last = stg + 1 == nStages;
             P.code = p.dCode + (p.stages.empty() ? 0 : p.stages[stg].codeOffset);
-            P.outVoice = (last && materialise) ? voiceOut + (offlineOut_ ? offlineOffset_ : 0) : nullptr;   // outputs and taps belong to the last stage
+            P.outVoice = (last && materialise) ? voiceOut + outOffset : nullptr;   // outputs and taps belong to the last stage
+            P.inShared = inShared ? inShared + inOffset : nullptr;
+            P.inVoice = inVoice ? inVoice + inOffset : nullptr;
             P.mixPartial = (last && mix) ? partialOut : nullptr;
             std::pair<cudaEvent_t, cudaEvent_t> ev{nullptr, nullptr};
             if (timeKernels_) {
@@ -2626,7 +2641,7 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
                     epi.gain0 = rd.gain0; epi.step = rd.step; epi.target = rd.target; epi.channel = rd.channel;
                     epi.nOut = P.nOut; epi.blockSize = blockSize_;
                     epi.mixPartial = mix ? partialOut : nullptr; epi.tileBase = P.tileBase;
-                    epi.outVoice = materialise ? voiceOut + (offlineOut_ ? offlineOffset_ : 0) : nullptr;
+                    epi.outVoice = materialise ? voiceOut + outOffset : nullptr;
                     epi.voice0 = P.voice0; epi.outStride = P.outStride; epi.outOffset = 0;
                 }
                 int offset = 0;
@@ -2641,9 +2656,9 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
                     }
                     const float* cin = cv.in;
                     int cinStride = blockSize_;
-                    if (cv.inChannel >= 0) {   // straight from the host input buffers: per-voice [voice][nIn][blockSize] or shared [nIn][blockSize]
-                        if (perVoiceIn) { cin = dInVoice_ + ((size_t) g.v0 * nIn + cv.inChannel) * blockSize_; cinStride = (int) nIn * blockSize_; }
-                        else { cin = dInShared_ + (size_t) cv.inChannel * blockSize_; cinStride = 0; }
+                    if (cv.inChannel >= 0) {   // straight from the host input buffers: per-voice [voice][nIn][inStride] or shared [nIn][inStride]
+                        if (perVoiceIn) { cin = inBase + ((size_t) g.v0 * nIn + cv.inChannel) * inStride + inOffset; cinStride = (int) nIn * inStride; }
+                        else { cin = inBase + (size_t) cv.inChannel * inStride + inOffset; cinStride = 0; }
                     }
                     if (!dry && !cuda(convolver_process_chunk(cs, cin, cinStride, cv.out, blockSize_, offset, n, stream_, epi), "convolver launch")) return rc::CudaError;
                     if (dry) { offset += n; continue; }
@@ -2704,8 +2719,8 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
         }
         steadyBuckets_.push_back(SteadyBucket{L, (int) descs.size(), total, maxSlots, maxState, maxParams, wpc, pipeStages, kv.first, smemOut});
         if (!dry && !cuda(pipeStages >= 1
-                              ? launch_render_groups_pipe(bb.dDescs, bb.dTileStart, (int) descs.size(), total, pipeStages, maxSlots, smemOut, maxState, maxParams, sampleTime_, offlineOut_ ? offlineOffset_ : 0, stream_, opt_.niter)
-                              : launch_render_groups(bb.dDescs, bb.dTileStart, (int) descs.size(), total, L, maxSlots, smemOut, maxState, maxParams, wpc, sampleTime_, offlineOut_ ? offlineOffset_ : 0, stream_, opt_.niter),
+                              ? launch_render_groups_pipe(bb.dDescs, bb.dTileStart, (int) descs.size(), total, pipeStages, maxSlots, smemOut, maxState, maxParams, sampleTime_, outOffset, inOffset, stream_, opt_.niter)
+                              : launch_render_groups(bb.dDescs, bb.dTileStart, (int) descs.size(), total, L, maxSlots, smemOut, maxState, maxParams, wpc, sampleTime_, outOffset, inOffset, stream_, opt_.niter),
                   "render groups kernel launch")) return rc::CudaError;
         if (timeKernels_) { cudaEventRecord(ev.second, stream_); timedEvents_.push_back(ev); }
         ++launches_;
@@ -2713,7 +2728,7 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
     // With the cross-GPU sum behind it, K2 leaves this rank's partial mix in PeerMix::own (K4 pushes it to the peers from there and
     // writes the total to the mix bus): no staging copy, no in-place hazard between K4's CTAs.
     const bool exchange = mix && allReduce && peerAttached_ && peer_.world > 1;
-    float* mixOut = dMix_;
+    float* mixOut = mixDst;
     if (exchange) {
         ++peerEpoch_;
         mixOut = peer_.own;
@@ -2726,9 +2741,11 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
     } else if (mix) {
         if (tileBase > 0) {
             auto ev = timedBegin();
-            if (!dry && !cuda(launch_mix_reduce(dPartial_, mixOut, dMixScratch_, dMixTickets_, tileBase, (int) nOut, blockSize_, (int) numSamples, stream_, exchange ? HostDeliver{} : takeDeliver()), "mix reduce launch")) return rc::CudaError;
+            if (!dry && !cuda(launch_mix_reduce(dPartial_, mixOut, exchange ? blockSize_ : mixStride, dMixScratch_, dMixTickets_, tileBase, (int) nOut, blockSize_, (int) numSamples, stream_, exchange ? HostDeliver{} : takeDeliver()), "mix reduce launch")) return rc::CudaError;
             if (timeKernels_) { cudaEventRecord(ev.second, stream_); timedMixEvents_.push_back(ev); }
             ++launches_;
+        } else if (offlineMix_) {   // the chunk's slots are reused: this block's column of every row is written on every block
+            if (!dry && !cuda(cudaMemset2DAsync(mixDst, sizeof(float) * mixStride, 0, sizeof(float) * blockSize_, nOut, stream_), "memset offline mix")) return rc::CudaError;
         } else {
             dmemset(mixOut, 0, sizeof(float) * nOut * blockSize_);
         }
@@ -2814,8 +2831,9 @@ int Engine::launchWide(size_t nOut, size_t numSamples, bool materialise, bool mi
     if (mix) {
         auto ev = timedBegin();
         const int nBig = (int) w.segs.size() - w.nSmall;
-        if (!cuda(launch_mix_reduce_wide(dPartial_, w.dRows, w.dSegs, w.nSmall, nBig, (int) nOut, dMix_, dWideScratch_, dWideTickets_, blockSize_,
-                                         (int) numSamples, stream_, takeDeliver()), "wide mix reduce launch")) return rc::CudaError;
+        float* const mixDst = offlineMix_ ? offlineMix_ + offlineOffset_ : dMix_;
+        if (!cuda(launch_mix_reduce_wide(dPartial_, w.dRows, w.dSegs, w.nSmall, nBig, (int) nOut, mixDst, offlineMix_ ? offlineStride_ : blockSize_,
+                                         dWideScratch_, dWideTickets_, blockSize_, (int) numSamples, stream_, takeDeliver()), "wide mix reduce launch")) return rc::CudaError;
         if (timeKernels_) { cudaEventRecord(ev.second, stream_); timedMixEvents_.push_back(ev); }
         launches_ += (w.nSmall > 0) + (nBig > 0);
     }
@@ -2871,71 +2889,135 @@ int Engine::renderOffline(size_t nOut, size_t numBlocks, float* hostOut, size_t 
     Lock lk(mu_);
     if (planOnly_) return fail(rc::CudaError, "plan-only runtime (no CUDA device): rendering is impossible, there is no CPU fallback");
     if (!hostOut || nOut == 0 || nOut > (size_t) MAX_OUT_CHANNELS) return fail(rc::BadArgument, "renderOffline: bad arguments");
-    dsetdev();
-    const size_t bs = (size_t) blockSize_, rows = (size_t) numVoices_ * nOut;
-    size_t C = chunkBlocks ? chunkBlocks : 8;
-    while (C > 1 && rows * C * bs * sizeof(float) > ((size_t) 256 << 20)) C >>= 1;          // two chunk buffers of at most 256 MiB each
-    if (C > numBlocks) C = std::max<size_t>(1, numBlocks);
-    // Chunk buffers: two on the device (rendered into back to back) and two PINNED on the host.  The user's buffer is pageable and
-    // strided ([row][numBlocks * bs]); a 2-D copy straight into it would be staged by the driver row by row, synchronously.  So a chunk
-    // leaves the device as ONE contiguous async copy into pinned memory on the copy stream, and this thread scatters the previous
-    // chunk's rows into the user's buffer while the GPU renders the next one.  The buffers are kept across calls.
-    const size_t chunkFloats = rows * C * bs;
-    if (chunkFloats > offlineChunkFloats_) {
-        dsync();
-        for (int i = 0; i < 2; ++i) {
-            if (offlineDev_[i]) cudaFree(offlineDev_[i]);
-            if (offlinePinned_[i]) cudaFreeHost(offlinePinned_[i]);
-            offlineDev_[i] = nullptr; offlinePinned_[i] = nullptr;
-        }
-        offlineChunkFloats_ = 0;
-        for (int i = 0; i < 2; ++i) {
-            if (!cuda(cudaMalloc((void**) &offlineDev_[i], chunkFloats * sizeof(float)), "cudaMalloc offline chunk")) return rc::CudaError;
-            if (!cuda(cudaMallocHost((void**) &offlinePinned_[i], chunkFloats * sizeof(float)), "cudaMallocHost offline chunk")) return rc::CudaError;
-        }
-        offlineChunkFloats_ = chunkFloats;
+    return offlineLoop(nullptr, 0, nullptr, nullptr, hostOut, nOut, numBlocks * (size_t) blockSize_, chunkBlocks, nullptr);
+}
+
+int Engine::processOffline(const float* const* in, size_t nIn, const float* inVoices, float* const* mixOut, float* voicesOut,
+                           size_t nOut, size_t numSamples, size_t chunkBlocks, const int64_t* sampleTime) {
+    Lock lk(mu_);
+    if (in && inVoices) return fail(rc::BadArgument, "processOffline: shared and per-voice inputs are exclusive");
+    if (nIn > 0 && !in && !inVoices) return fail(rc::BadArgument, "processOffline: nIn > 0 without inputs");
+    if (nOut == 0 || nOut > (size_t) MAX_WIDE_OUT_CHANNELS || (voicesOut && nOut > (size_t) MAX_OUT_CHANNELS))
+        return fail(rc::BadArgument, "processOffline: nOut must be 1..4096 (1..8 with per-voice outputs)");
+    if (processAllReduce_ && peerAttached_ && peer_.world > 1)
+        return fail(rc::BadArgument, "processOffline: the mix bus is not summed across GPUs offline (option process_allreduce = 0 renders this rank alone)");
+    if (planOnly_) return fail(rc::CudaError, "plan-only runtime (no CUDA device): rendering is impossible, there is no CPU fallback");
+    return offlineLoop(nIn ? in : nullptr, nIn, nIn ? inVoices : nullptr, mixOut, voicesOut, nOut, numSamples, chunkBlocks, sampleTime);
+}
+
+int Engine::ensureOfflineBuf(OfflineBuf& b, size_t floats) {
+    if (floats <= b.floats) return rc::Ok;
+    dsync();
+    for (int i = 0; i < 2; ++i) {
+        if (b.dev[i]) cudaFree(b.dev[i]);
+        if (b.pinned[i]) cudaFreeHost(b.pinned[i]);
+        b.dev[i] = nullptr; b.pinned[i] = nullptr;
     }
-    cudaStream_t copyStream = nullptr;
-    cudaEvent_t rendered[2] = {nullptr, nullptr}, copied[2] = {nullptr, nullptr};
+    b.floats = 0;
+    for (int i = 0; i < 2; ++i) {
+        if (!cuda(cudaMalloc((void**) &b.dev[i], floats * sizeof(float)), "cudaMalloc offline chunk")) return rc::CudaError;
+        if (!cuda(cudaMallocHost((void**) &b.pinned[i], floats * sizeof(float)), "cudaMallocHost offline chunk")) return rc::CudaError;
+    }
+    b.floats = floats;
+    return rc::Ok;
+}
+
+// The chunk loop of both offline entry points (the engine lock is held).  Blocks are enqueued back to back with no host synchronisation in
+// between; chunk buffers of C blocks per row carry the inputs up and the outputs down, two of each on the device and two PINNED on the host.
+// The user's buffers are pageable and strided; a 2-D copy straight from or into them would be staged by the driver row by row,
+// synchronously.  So a chunk travels as ONE contiguous async copy between pinned and device memory, and this thread moves rows between the
+// user's buffers and pinned memory while the GPU renders: it fills chunk k + 1's inputs (uploaded on their own stream) and scatters
+// chunk k - 1's outputs while chunk k renders.
+int Engine::offlineLoop(const float* const* in, size_t nIn, const float* inVoices, float* const* mixOut, float* voicesOut,
+                        size_t nOut, size_t numSamples, size_t chunkBlocks, const int64_t* sampleTime) {
+    dsetdev();
+    const size_t bs = (size_t) blockSize_, numBlocks = (numSamples + bs - 1) / bs;
+    if (numBlocks == 0) return rc::Ok;
+    const bool perVoiceIn = inVoices != nullptr;
+    const size_t inRows = perVoiceIn ? (size_t) numVoices_ * nIn : (in ? nIn : 0);
+    const size_t outRows = voicesOut ? (size_t) numVoices_ * nOut : 0, mixRows = mixOut ? nOut : 0;
+    const size_t maxRows = std::max(inRows, std::max(outRows, mixRows));
+    size_t C = chunkBlocks ? chunkBlocks : 8;
+    while (C > 1 && maxRows * C * bs * sizeof(float) > ((size_t) 256 << 20)) C >>= 1;       // two chunk buffers of at most 256 MiB each
+    if (C > numBlocks) C = numBlocks;
+    const size_t W = C * bs, numChunks = (numBlocks + C - 1) / C;                           // W: floats per chunk row
+    int r = rc::Ok;
+    if (outRows && (r = ensureOfflineBuf(offOut_, outRows * W)) != rc::Ok) return r;
+    if (inRows && (r = ensureOfflineBuf(offIn_, inRows * W)) != rc::Ok) return r;
+    if (mixRows && (r = ensureOfflineBuf(offMix_, mixRows * W)) != rc::Ok) return r;
+    cudaStream_t copyStream = nullptr, upStream = nullptr;
+    cudaEvent_t rendered[2] = {nullptr, nullptr}, copied[2] = {nullptr, nullptr}, uploaded[2] = {nullptr, nullptr};
     int rcode = rc::Ok;
     for (int i = 0; i < 2; ++i) {
-        cudaMemsetAsync(offlineDev_[i], 0, chunkFloats * sizeof(float), stream_);               // voices without a render sequence stay silent
+        if (outRows) cudaMemsetAsync(offOut_.dev[i], 0, outRows * W * sizeof(float), stream_);    // voices without a render sequence stay silent
         cudaEventCreateWithFlags(&rendered[i], cudaEventDisableTiming);
         cudaEventCreateWithFlags(&copied[i], cudaEventDisableTiming);
+        cudaEventCreateWithFlags(&uploaded[i], cudaEventDisableTiming);
     }
     cudaStreamCreateWithFlags(&copyStream, cudaStreamNonBlocking);
+    if (inRows) cudaStreamCreateWithFlags(&upStream, cudaStreamNonBlocking);
     steadyValid_ = false;
+    auto stage = [&](size_t chunk) -> bool {       // user rows -> pinned slot (zero past numSamples) -> device slot
+        const int slot = (int) (chunk & 1);
+        if (!cuda(cudaEventSynchronize(uploaded[slot]), "wait for an offline input upload")) return false;   // the upload two chunks back
+        float* const dst = offIn_.pinned[slot];
+        const size_t s0 = chunk * W, n = std::min(W, numSamples - s0);
+        for (size_t row = 0; row < inRows; ++row) {
+            std::memcpy(dst + row * W, perVoiceIn ? inVoices + row * numSamples + s0 : in[row] + s0, n * sizeof(float));
+            if (n < W) std::memset(dst + row * W + n, 0, (W - n) * sizeof(float));
+        }
+        cudaStreamWaitEvent(upStream, rendered[slot], 0);                                      // the chunk two back no longer reads the device slot
+        if (!cuda(cudaMemcpyAsync(offIn_.dev[slot], dst, inRows * W * sizeof(float), cudaMemcpyHostToDevice, upStream), "H2D offline input chunk")) return false;
+        return cuda(cudaEventRecord(uploaded[slot], upStream), "record an offline input upload");
+    };
     struct Pending { bool valid = false; size_t chunk = 0, blocks = 0; int slot = 0; } prev;
-    auto scatter = [&](const Pending& pc) {          // pinned chunk [row][C * bs] -> user rows
+    auto scatter = [&](const Pending& pc) {          // pinned chunk [row][W] -> user rows, truncated to numSamples
         if (!pc.valid) return;
         if (!cuda(cudaEventSynchronize(copied[pc.slot]), "wait for an offline chunk")) { rcode = rc::CudaError; return; }
-        const size_t width = pc.blocks * bs;
-        for (size_t r = 0; r < rows; ++r)
-            std::memcpy(hostOut + r * numBlocks * bs + pc.chunk * C * bs, offlinePinned_[pc.slot] + r * C * bs, width * sizeof(float));
+        const size_t s0 = pc.chunk * W, width = std::min(pc.blocks * bs, numSamples - s0);
+        for (size_t row = 0; row < outRows; ++row)
+            std::memcpy(voicesOut + row * numSamples + s0, offOut_.pinned[pc.slot] + row * W, width * sizeof(float));
+        for (size_t c = 0; c < mixRows; ++c)
+            std::memcpy(mixOut[c] + s0, offMix_.pinned[pc.slot] + c * W, width * sizeof(float));
     };
+    if (inRows && !stage(0)) rcode = rc::CudaError;
     for (size_t b = 0; b < numBlocks && rcode == rc::Ok; ++b) {
         const size_t chunk = b / C, inChunk = b % C;
         const int slot = (int) (chunk & 1);
-        if (inChunk == 0 && chunk >= 2) cudaStreamWaitEvent(stream_, copied[slot], 0);          // the chunk two back has left this device buffer
-        offlineOut_ = offlineDev_[slot]; offlineStride_ = (int) (C * bs); offlineOffset_ = (int) (inChunk * bs);
-        rcode = enqueueBlock(0, nOut, bs, false, true, false);
+        if (inChunk == 0) {
+            if (chunk >= 2) cudaStreamWaitEvent(stream_, copied[slot], 0);                       // the chunk two back has left these device buffers
+            if (inRows) cudaStreamWaitEvent(stream_, uploaded[slot], 0);                         // this chunk's inputs have arrived
+        }
+        if (sampleTime) sampleTime_ = *sampleTime + (int64_t) (b * bs);                          // as process() with userData, block by block
+        offlineOut_ = outRows ? offOut_.dev[slot] : nullptr;
+        offlineIn_ = inRows ? offIn_.dev[slot] : nullptr;
+        offlineMix_ = mixRows ? offMix_.dev[slot] : nullptr;
+        offlineStride_ = (int) W; offlineOffset_ = (int) (inChunk * bs);
+        rcode = enqueueBlock(nIn, nOut, bs, perVoiceIn, outRows != 0, mixRows != 0);
         const bool lastOfChunk = inChunk + 1 == C || b + 1 == numBlocks;
         if (rcode == rc::Ok && lastOfChunk) {
-            // the pinned buffer of this slot was scattered when chunk - 1 was enqueued (below), i.e. before this copy is issued
+            // the pinned buffers of this slot were scattered when chunk - 1 was enqueued (below), i.e. before these copies are issued
             cudaEventRecord(rendered[slot], stream_);
             cudaStreamWaitEvent(copyStream, rendered[slot], 0);
-            if (!cuda(cudaMemcpyAsync(offlinePinned_[slot], offlineDev_[slot], chunkFloats * sizeof(float), cudaMemcpyDeviceToHost, copyStream), "D2H offline chunk")) rcode = rc::CudaError;
+            if (outRows && !cuda(cudaMemcpyAsync(offOut_.pinned[slot], offOut_.dev[slot], outRows * W * sizeof(float), cudaMemcpyDeviceToHost, copyStream), "D2H offline chunk")) rcode = rc::CudaError;
+            if (mixRows && !cuda(cudaMemcpyAsync(offMix_.pinned[slot], offMix_.dev[slot], mixRows * W * sizeof(float), cudaMemcpyDeviceToHost, copyStream), "D2H offline mix chunk")) rcode = rc::CudaError;
             cudaEventRecord(copied[slot], copyStream);
+            if (rcode == rc::Ok && inRows && chunk + 1 < numChunks && !stage(chunk + 1)) rcode = rc::CudaError;   // overlaps with this chunk's render
             Pending cur; cur.valid = true; cur.chunk = chunk; cur.blocks = inChunk + 1; cur.slot = slot;
             scatter(prev);                                                                      // overlaps with the GPU rendering what was just enqueued
             prev = cur;
         }
     }
-    scatter(prev);
-    offlineOut_ = nullptr; offlineStride_ = 0; offlineOffset_ = 0; steadyValid_ = false;
+    if (rcode == rc::Ok) scatter(prev);
+    offlineOut_ = nullptr; offlineIn_ = nullptr; offlineMix_ = nullptr; offlineStride_ = 0; offlineOffset_ = 0; steadyValid_ = false;
     cudaStreamSynchronize(stream_);
     if (copyStream) { cudaStreamSynchronize(copyStream); cudaStreamDestroy(copyStream); }
-    for (int i = 0; i < 2; ++i) { if (rendered[i]) cudaEventDestroy(rendered[i]); if (copied[i]) cudaEventDestroy(copied[i]); }
+    if (upStream) { cudaStreamSynchronize(upStream); cudaStreamDestroy(upStream); }
+    for (int i = 0; i < 2; ++i) {
+        if (rendered[i]) cudaEventDestroy(rendered[i]);
+        if (copied[i]) cudaEventDestroy(copied[i]);
+        if (uploaded[i]) cudaEventDestroy(uploaded[i]);
+    }
     return rcode;
 }
 

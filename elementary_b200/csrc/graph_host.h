@@ -222,6 +222,13 @@ public:
     // of `chunkBlocks` blocks ([voice][nOut][chunk] on the device), and finished chunks travel to hostOut[voice][nOut][numBlocks *
     // blockSize] on a copy stream while the next chunk renders.  The reference does the same job with OfflineRenderer.process in a loop.
     int renderOffline(size_t nOut, size_t numBlocks, float* hostOut, size_t chunkBlocks);
+    // OfflineRenderer.process(inputs, outputs) (js/packages/offline-renderer/index.ts:87-133): ceil(numSamples / blockSize) full blocks
+    // through the same chunk loop, with inputs (shared in[c][numSamples] or per-voice inVoices[voice][nIn][numSamples], zero past
+    // numSamples) going up through chunk buffers too, and the mix bus (mixOut[c][numSamples]) and / or per-voice outputs
+    // (voicesOut[voice][nOut][numSamples]) coming back, truncated to numSamples.  Block k of the mix is what process() returns for the same
+    // block; sampleTime: as process()'s, for the first block (block k gets *sampleTime + k * blockSize).
+    int processOffline(const float* const* in, size_t nIn, const float* inVoices, float* const* mixOut, float* voicesOut,
+                       size_t nOut, size_t numSamples, size_t chunkBlocks, const int64_t* sampleTime);
 
     // Cross-GPU mix bus (SURVEY.md §8e): peerExport() allocates this rank's exchange buffer and returns its CUDA IPC handle
     // (64 bytes); peerAttach() maps the buffers of all ranks (handles = world x 64 bytes, in rank order).  Afterwards
@@ -323,7 +330,12 @@ private:
     bool hostDeliver_ = true, processAllReduce_ = true;   // options "host_deliver", "process_allreduce"
     bool deliverArmed_ = false, deliverLaunched_ = false;
     HostDeliver takeDeliver();
-    float* offlineDev_[2] = {nullptr, nullptr}; float* offlinePinned_[2] = {nullptr, nullptr}; size_t offlineChunkFloats_ = 0;   // renderOffline chunk buffers, kept across calls
+    // Offline chunk buffers, kept across calls: two on the device (rendered into / uploaded to back to back), two pinned on the host
+    struct OfflineBuf { float* dev[2] = {nullptr, nullptr}; float* pinned[2] = {nullptr, nullptr}; size_t floats = 0; };
+    OfflineBuf offOut_, offIn_, offMix_;  // per-voice outputs [voice][nOut][C * bs], inputs [nIn][C * bs] or [voice][nIn][C * bs], mix [nOut][C * bs]
+    int ensureOfflineBuf(OfflineBuf& b, size_t floats);
+    int offlineLoop(const float* const* in, size_t nIn, const float* inVoices, float* const* mixOut, float* voicesOut,
+                    size_t nOut, size_t numSamples, size_t chunkBlocks, const int64_t* sampleTime);
     size_t curNOut_ = 0;
     struct BatchBuffers { LaunchParams* dDescs = nullptr; int* dTileStart = nullptr; size_t capGroups = 0; std::vector<char> lastDescs; };
     std::map<int, BatchBuffers> batch_;   // per tile width
@@ -335,7 +347,7 @@ private:
     static constexpr int PIPE_BUCKET = 1000;   // bucket key = tile width (+ PIPE_BUCKET for pipelined one-voice programs)
     std::vector<SteadyBucket> steadyBuckets_;
     bool steadyValid_ = false;
-    size_t steadyKey_[6] = {0, 0, 0, 0, 0, 0};
+    size_t steadyKey_[7] = {0, 0, 0, 0, 0, 0, 0};
     int steadyTiles_ = 0;
     // Wide mix bus (nOut > MAX_OUT_CHANNELS, DESIGN.md section 3): each voice group writes compact partial rows for the channels its
     // roots aim at only (mix channels, ascending), per-voice outputs go to a compact [voice][mix channel] buffer and are scattered to
@@ -361,7 +373,9 @@ private:
     int launchWide(size_t nOut, size_t numSamples, bool materialise, bool mix);
     // the mix channels of a program: distinct channels in [0, nOut) of all its roots, running or fading, ascending
     std::vector<int> mixChannels(const Group& g, const Program& p, size_t nOut) const;
-    float* offlineOut_ = nullptr; int offlineStride_ = 0, offlineOffset_ = 0;   // renderOffline: where materialised outputs go instead of dOutVoice_
+    // Offline blocks: where materialised outputs, inputs and the mix bus are instead of dOutVoice_, dInShared_ / dInVoice_ and dMix_ (chunk
+    // buffers of rows of offlineStride_ floats; this block's column starts at offlineOffset_)
+    float* offlineOut_ = nullptr; const float* offlineIn_ = nullptr; float* offlineMix_ = nullptr; int offlineStride_ = 0, offlineOffset_ = 0;
 
     // K4 state
     void* dExchange_ = nullptr; size_t exchangeBytes_ = 0; size_t exchangeFlagOffset_ = 0, exchangeOwnOffset_ = 0;

@@ -13,17 +13,19 @@ int render_delay_buf_floats(int nDelayBuf, int tileWidth, int niterOverride);   
 struct SpecKernel;   // spec_host.h: K1 compiled at run time against one program (nullptr = the built-in interpreter)
 cudaError_t launch_render_block(const LaunchParams& P, int warpsPerCta, int niterOverride, cudaStream_t stream, const SpecKernel* spec = nullptr);
 
-// K1 for many voice groups of one tile geometry in one launch (descs / tileStart are device pointers).
+// K1 for many voice groups of one tile geometry in one launch (descs / tileStart are device pointers).  outOffset / inOffset: the
+// column of every output / input row the block starts at (an offline chunk holds several blocks per row; 0 otherwise).
 cudaError_t launch_render_groups(const LaunchParams* descs, const int* tileStart, int nGroups, int totalTiles, int tileWidth,
-                                 int maxSlots, int nOut, int maxStateRows, int maxParams, int warpsPerCta, long long sampleTime, int outOffset, cudaStream_t stream,
+                                 int maxSlots, int nOut, int maxStateRows, int maxParams, int warpsPerCta, long long sampleTime, int outOffset, int inOffset, cudaStream_t stream,
                                  int niterOverride = 0);
 
 // K1 for many ONE-VOICE graphs whose programs were cut into pipeline stages (LaunchParams::pipeW): one CTA of `stages` warps per graph.
 cudaError_t launch_render_groups_pipe(const LaunchParams* descs, const int* tileStart, int nGroups, int totalTiles, int stages,
-                                      int maxSlots, int nOut, int maxStateRows, int maxParams, long long sampleTime, int outOffset, cudaStream_t stream,
+                                      int maxSlots, int nOut, int maxStateRows, int maxParams, long long sampleTime, int outOffset, int inOffset, cudaStream_t stream,
                                       int niterOverride = 0);
 
-// K2: deterministic reduction of per-tile partial mixes into the [nOut][blockSize] mix bus.
+// K2: deterministic reduction of per-tile partial mixes into the mix bus, channel c at out + c * outStride (blockSize for the mix bus
+// of one block; an offline chunk's column otherwise; a host-delivery copy always has pitch blockSize).
 // scratch: [MIX_REDUCE_MAX_GROUPS][nOut][blockSize] floats, tickets: [nOut * ceil(blockSize/32)] zeroed counters (both may be null:
 // single-pass reduction).
 constexpr int MIX_REDUCE_MAX_GROUPS = 16;
@@ -36,11 +38,11 @@ struct HostDeliver {
     unsigned int* done = nullptr;    // device counter, zero between launches
     uint32_t seq = 0;
 };
-cudaError_t launch_mix_reduce(const float* partial, float* out, float* scratch, unsigned int* tickets, int nTiles, int nOut, int blockSize,
-                              int numSamples, cudaStream_t stream, HostDeliver hd = HostDeliver{});
+cudaError_t launch_mix_reduce(const float* partial, float* out, int outStride, float* scratch, unsigned int* tickets, int nTiles, int nOut,
+                              int blockSize, int numSamples, cudaStream_t stream, HostDeliver hd = HostDeliver{});
 
 // K2w (mix_wide_kernel.cu): the mix bus for nOut > MAX_OUT_CHANNELS from COMPACT partial rows [row][blockSize].  Channel c sums its row
-// list rows[rowPtr_c ...] with K2's tree; a segment is one tile group of one channel.  Every channel in [0, nOut) has at least one
+// list rows[rowPtr_c ...] with K2's tree into out + c * outStride (pitch as for K2); a segment is one tile group of one channel.  Every channel in [0, nOut) has at least one
 // segment (a channel without rows has one empty segment, which writes +0.0).
 constexpr int MAX_WIDE_OUT_CHANNELS = 4096;   // output channels of the compact mix bus; a call with more returns -2
 struct WideSeg {
@@ -52,7 +54,7 @@ struct WideSeg {
 // segs: the nSmall segments of fewer than WIDE_BIG_ROWS rows (a warp each), then the nBig larger ones (a CTA of 32 warps each).
 constexpr int WIDE_BIG_ROWS = 128;
 cudaError_t launch_mix_reduce_wide(const float* partial, const int* rows, const WideSeg* segs, int nSmall, int nBig, int nOut, float* out,
-                                   float* scratch, unsigned int* tickets, int blockSize, int numSamples, cudaStream_t stream,
+                                   int outStride, float* scratch, unsigned int* tickets, int blockSize, int numSamples, cudaStream_t stream,
                                    HostDeliver hd = HostDeliver{});
 // Per-voice outputs of the wide path: compact row r [blockSize] -> row dstRow[r] of out ([voice][nOut][blockSize]), numSamples samples.
 cudaError_t launch_voice_out_scatter(const float* compact, const int* dstRow, int nRows, float* out, int blockSize, int numSamples, cudaStream_t stream);

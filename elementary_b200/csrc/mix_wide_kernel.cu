@@ -74,10 +74,10 @@ __device__ __forceinline__ void wide_lane_sums(const float* __restrict__ col, co
 // warp that arrives last at the (channel, chunk) ticket, 0 + s_0 + ... + s_(G-1) in group order.  Then the host-delivery arrival.
 __device__ __forceinline__ void wide_finish(const WideSeg& sg, float v, int chunk, int chunksPerBlock, int s, bool live, int lane,
                                             float* __restrict__ out, float* __restrict__ scratch, unsigned int* __restrict__ tickets,
-                                            int blockSize, unsigned int nFinal, const HostDeliver& hd) {
-    const size_t o = (size_t) sg.channel * blockSize + s;
+                                            int blockSize, int outStride, unsigned int nFinal, const HostDeliver& hd) {
+    const size_t o = (size_t) sg.channel * outStride + s, oh = (size_t) sg.channel * blockSize + s;
     if (sg.groups == 1) {
-        if (live) { out[o] = v; if (hd.out) hd.out[o] = v; }
+        if (live) { out[o] = v; if (hd.out) hd.out[oh] = v; }
         if (hd.out) wide_deliver_arrive(hd, nFinal, lane);
         return;
     }
@@ -97,7 +97,7 @@ __device__ __forceinline__ void wide_finish(const WideSeg& sg, float v, int chun
         float w = 0.0f;
         for (int k = 0; k < sg.groups; ++k) w += __ldcg(scratch + (size_t) (sg.scratch + k) * blockSize + s);
         out[o] = w;
-        if (hd.out) hd.out[o] = w;
+        if (hd.out) hd.out[oh] = w;
     }
     if (hd.out) wide_deliver_arrive(hd, nFinal, lane);
 }
@@ -106,7 +106,7 @@ __device__ __forceinline__ void wide_finish(const WideSeg& sg, float v, int chun
 __global__ void __launch_bounds__(32 * WIDE_WARPS) mix_reduce_wide_kernel(const float* __restrict__ partial, const int* __restrict__ rows,
                                                                           const WideSeg* __restrict__ segs, int nItems, int chunks, int chunksPerBlock,
                                                                           float* __restrict__ out, float* __restrict__ scratch,
-                                                                          unsigned int* __restrict__ tickets, int blockSize, int numSamples,
+                                                                          unsigned int* __restrict__ tickets, int blockSize, int outStride, int numSamples,
                                                                           unsigned int nFinal, const HostDeliver hd) {
     const int item = blockIdx.x * WIDE_WARPS + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
@@ -127,7 +127,7 @@ __global__ void __launch_bounds__(32 * WIDE_WARPS) mix_reduce_wide_kernel(const 
         for (int q = 0; q < WIDE_LANE_BLOCK; ++q)
             if (jb + q < nl) v += sums[q];
     }
-    wide_finish(sg, v, chunk, chunksPerBlock, s, live, lane, out, scratch, tickets, blockSize, nFinal, hd);
+    wide_finish(sg, v, chunk, chunksPerBlock, s, live, lane, out, scratch, tickets, blockSize, outStride, nFinal, hd);
 }
 
 // Segments of WIDE_BIG_ROWS rows or more: one CTA per (segment, chunk); warp w forms the sums of row lanes w * WIDE_BIG_LANES ...
@@ -135,7 +135,7 @@ __global__ void __launch_bounds__(32 * WIDE_WARPS) mix_reduce_wide_kernel(const 
 __global__ void __launch_bounds__(32 * WIDE_BIG_WARPS) mix_reduce_wide_big_kernel(const float* __restrict__ partial, const int* __restrict__ rows,
                                                                                   const WideSeg* __restrict__ segs, int chunks, int chunksPerBlock,
                                                                                   float* __restrict__ out, float* __restrict__ scratch,
-                                                                                  unsigned int* __restrict__ tickets, int blockSize, int numSamples,
+                                                                                  unsigned int* __restrict__ tickets, int blockSize, int outStride, int numSamples,
                                                                                   unsigned int nFinal, const HostDeliver hd) {
     __shared__ float laneSum[32][33];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -152,7 +152,7 @@ __global__ void __launch_bounds__(32 * WIDE_BIG_WARPS) mix_reduce_wide_big_kerne
     if (warp != 0) return;
     float v = 0.0f;
     for (int j = 0; j < 32; ++j) v += laneSum[j][lane];           // every lane has items (>= 32 rows): 0 + lane 0 + ... + lane 31
-    wide_finish(sg, v, chunk, chunksPerBlock, s, live, lane, out, scratch, tickets, blockSize, nFinal, hd);
+    wide_finish(sg, v, chunk, chunksPerBlock, s, live, lane, out, scratch, tickets, blockSize, outStride, nFinal, hd);
 }
 
 // Per-voice outputs of the wide path: the compact rows [row][blockSize] go to out[dstRow[row]] ([voice][nOut][blockSize]); the
@@ -167,20 +167,20 @@ __global__ void __launch_bounds__(128) voice_out_scatter_kernel(const float* __r
 }
 
 cudaError_t launch_mix_reduce_wide(const float* partial, const int* rows, const WideSeg* segs, int nSmall, int nBig, int nOut, float* out,
-                                   float* scratch, unsigned int* tickets, int blockSize, int numSamples, cudaStream_t stream, HostDeliver hd) {
+                                   int outStride, float* scratch, unsigned int* tickets, int blockSize, int numSamples, cudaStream_t stream, HostDeliver hd) {
     const int chunks = numSamples > 0 ? (numSamples + 31) / 32 : 1;
     const int chunksPerBlock = (blockSize + 31) / 32;
     const unsigned int nFinal = (unsigned int) (nOut * chunks);   // (channel, chunk) pairs: the host-delivery arrivals of both launches
     if (nSmall > 0) {
         const int nItems = nSmall * chunks;
         mix_reduce_wide_kernel<<<(nItems + WIDE_WARPS - 1) / WIDE_WARPS, 32 * WIDE_WARPS, 0, stream>>>(
-            partial, rows, segs, nItems, chunks, chunksPerBlock, out, scratch, tickets, blockSize, numSamples, nFinal, hd);
+            partial, rows, segs, nItems, chunks, chunksPerBlock, out, scratch, tickets, blockSize, outStride, numSamples, nFinal, hd);
         const cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }
     if (nBig > 0) {
         mix_reduce_wide_big_kernel<<<nBig * chunks, 32 * WIDE_BIG_WARPS, 0, stream>>>(
-            partial, rows, segs + nSmall, chunks, chunksPerBlock, out, scratch, tickets, blockSize, numSamples, nFinal, hd);
+            partial, rows, segs + nSmall, chunks, chunksPerBlock, out, scratch, tickets, blockSize, outStride, numSamples, nFinal, hd);
         return cudaGetLastError();
     }
     return cudaSuccess;

@@ -534,7 +534,7 @@ __device__ unsigned long long g_opprof[2 * 64];
 // warps of the CTA share the graph's shared-memory area and hand sample tiles on through progress counters (see LaunchParams).
 template <int NITER, int LOGL, bool PIPE = false>
 __device__ __forceinline__ void render_tile(const LaunchParams& P, const int tile, const int perWarp, const long long sampleTime, const int outOffset,
-                                            const int stage = 0) {
+                                            const int inOffset, const int stage = 0) {
     constexpr int L = 1 << LOGL;          // voices per warp
     constexpr int E = 32 * NITER;         // elements per sample tile
     constexpr int T = E >> LOGL;          // samples per tile
@@ -961,7 +961,7 @@ __global__ void EB_BOUNDS render_block_kernel(const __grid_constant__ LaunchPara
         stage_table_tma(P.tableSrc, P.tableFloats, g_smem + P.tableSmem, reinterpret_cast<uint64_t*>(g_smem + P.tableSmem + P.tableFloats));
     const int tile = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (tile >= ((P.nv + (1 << LOGL) - 1) >> LOGL)) return;   // whole warp leaves together
-    render_tile<NITER, LOGL>(P, tile, perWarp, P.sampleTime, 0);
+    render_tile<NITER, LOGL>(P, tile, perWarp, P.sampleTime, 0, 0);   // (offline chunks: the host pre-offsets the I/O pointers)
 }
 
 // Many voice groups (different graphs) of the same tile geometry in ONE launch: warp w finds its group by binary
@@ -969,7 +969,8 @@ __global__ void EB_BOUNDS render_block_kernel(const __grid_constant__ LaunchPara
 // thousands of small heterogeneous graphs (BASELINE config 5) run concurrently instead of one launch each.
 template <int NITER, int LOGL>
 __global__ void EB_BOUNDS render_groups_kernel(const LaunchParams* __restrict__ descs, const int* __restrict__ tileStart,
-                                                const int nGroups, const int totalTiles, const int perWarp, const long long sampleTime, const int outOffset) {
+                                                const int nGroups, const int totalTiles, const int perWarp, const long long sampleTime, const int outOffset,
+                                                const int inOffset) {
     const int w = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (w >= totalTiles) return;
     int lo = 0, hi = nGroups - 1;                      // largest g with tileStart[g] <= w
@@ -977,7 +978,8 @@ __global__ void EB_BOUNDS render_groups_kernel(const LaunchParams* __restrict__ 
         const int mid = (lo + hi + 1) >> 1;
         if (__ldg(tileStart + mid) <= w) lo = mid; else hi = mid - 1;
     }
-    render_tile<NITER, LOGL>(descs[lo], w - __ldg(tileStart + lo), perWarp, sampleTime, outOffset);   // the sample clock travels as an argument: the descriptors of a steady engine never change
+    // the sample clock and the I/O columns of an offline chunk travel as arguments: the descriptors of a steady engine never change
+    render_tile<NITER, LOGL>(descs[lo], w - __ldg(tileStart + lo), perWarp, sampleTime, outOffset, inOffset);
 }
 
 // The same for one-voice graphs whose programs the host cut into pipeline stages (LaunchParams::pipeW): ONE CTA per graph, warp w of
@@ -987,7 +989,7 @@ __global__ void EB_BOUNDS render_groups_kernel(const LaunchParams* __restrict__ 
 template <int NITER>
 __global__ void __launch_bounds__(32 * MAX_PIPE, 8) render_groups_pipe_kernel(const LaunchParams* __restrict__ descs, const int* __restrict__ tileStart,
                                                                               const int nGroups, const int totalTiles, const int perGraph,
-                                                                              const long long sampleTime, const int outOffset) {
+                                                                              const long long sampleTime, const int outOffset, const int inOffset) {
     const int w = blockIdx.x;                          // one-voice tiles: tile index == CTA index
     const int stage = threadIdx.x >> 5;
     if (threadIdx.x < MAX_PIPE) reinterpret_cast<volatile int*>(g_smem + perGraph)[threadIdx.x] = 0;   // progress counters
@@ -1000,7 +1002,7 @@ __global__ void __launch_bounds__(32 * MAX_PIPE, 8) render_groups_pipe_kernel(co
     }
     const LaunchParams& P = descs[lo];
     if (stage >= max(1, P.pipeW)) return;              // (whole warps leave; no CTA-wide barrier follows)
-    render_tile<NITER, 0, true>(P, w - __ldg(tileStart + lo), perGraph, sampleTime, outOffset, stage);
+    render_tile<NITER, 0, true>(P, w - __ldg(tileStart + lo), perGraph, sampleTime, outOffset, inOffset, stage);
 }
 
 #ifndef __CUDACC_RTC__   // K2, K4 and the host launchers are not needed by a run-time compiled specialisation of K1
@@ -1030,7 +1032,8 @@ __device__ __forceinline__ void host_deliver_arrive(const HostDeliver& hd, unsig
 }
 
 __global__ void __launch_bounds__(1024) mix_reduce_kernel(const float* __restrict__ partial, float* __restrict__ out, float* __restrict__ scratch,
-                                                          unsigned int* __restrict__ tickets, int nTiles, int nOut, int blockSize, int numSamples, const HostDeliver hd) {
+                                                          unsigned int* __restrict__ tickets, int nTiles, int nOut, int blockSize, int outStride, int numSamples,
+                                                          const HostDeliver hd) {
     __shared__ float red[32][33];
     __shared__ bool last;
     const int sx = threadIdx.x & 31, gy = threadIdx.x >> 5;       // 32 samples x 32 tile lanes
@@ -1053,7 +1056,7 @@ __global__ void __launch_bounds__(1024) mix_reduce_kernel(const float* __restric
     if (gy == 0) {
         float v = 0.0f;
         for (int k = 0; k < 32; ++k) v += red[k][sx];
-        if (G == 1) { if (s < numSamples) { out[(size_t) ch * blockSize + s] = v; if (hd.out) hd.out[(size_t) ch * blockSize + s] = v; } }
+        if (G == 1) { if (s < numSamples) { out[(size_t) ch * outStride + s] = v; if (hd.out) hd.out[(size_t) ch * blockSize + s] = v; } }
         else if (s < numSamples) scratch[((size_t) g * nOut + ch) * blockSize + s] = v;
     }
     if (G == 1) {
@@ -1072,7 +1075,7 @@ __global__ void __launch_bounds__(1024) mix_reduce_kernel(const float* __restric
         __threadfence();
         float v = 0.0f;
         for (int k = 0; k < G; ++k) v += __ldcg(scratch + ((size_t) k * nOut + ch) * blockSize + s);
-        out[(size_t) ch * blockSize + s] = v;
+        out[(size_t) ch * outStride + s] = v;
         if (hd.out) hd.out[(size_t) ch * blockSize + s] = v;
     }
     if (last && hd.out) host_deliver_arrive(hd, gridDim.x);   // `last` is uniform over the CTA: one finishing CTA per chunk
@@ -1118,11 +1121,11 @@ static cudaError_t launch_render_block_geometry(const LaunchParams& P, int L, in
 
 template <int NITER, int LOGL>
 static cudaError_t launch_groups_impl(const LaunchParams* descs, const int* tileStart, int nGroups, int totalTiles,
-                                      int grid, int threads, size_t smem, long long sampleTime, int outOffset, cudaStream_t stream) {
+                                      int grid, int threads, size_t smem, long long sampleTime, int outOffset, int inOffset, cudaStream_t stream) {
     cudaError_t e = cudaFuncSetAttribute(render_groups_kernel<NITER, LOGL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
     if (e != cudaSuccess) return e;
     render_groups_kernel<NITER, LOGL><<<grid, threads, smem, stream>>>(descs, tileStart, nGroups, totalTiles,
-                                                                          (int) (smem / sizeof(float) / (threads / 32)), sampleTime, outOffset);
+                                                                          (int) (smem / sizeof(float) / (threads / 32)), sampleTime, outOffset, inOffset);
     return cudaGetLastError();
 }
 
@@ -1162,7 +1165,7 @@ static cudaError_t launch_render_block_geometry(const LaunchParams& P, int L, in
 
 // descs / tileStart are DEVICE pointers; maxSlots etc. are the maxima over the groups (uniform shared-memory carve-up).
 cudaError_t launch_render_groups(const LaunchParams* descs, const int* tileStart, int nGroups, int totalTiles, int tileWidth,
-                                 int maxSlots, int nOut, int maxStateRows, int maxParams, int warpsPerCta, long long sampleTime, int outOffset, cudaStream_t stream,
+                                 int maxSlots, int nOut, int maxStateRows, int maxParams, int warpsPerCta, long long sampleTime, int outOffset, int inOffset, cudaStream_t stream,
                                  int niterOverride) {
     if (totalTiles <= 0) return cudaSuccess;
     const int grid = (totalTiles + warpsPerCta - 1) / warpsPerCta;
@@ -1171,24 +1174,24 @@ cudaError_t launch_render_groups(const LaunchParams* descs, const int* tileStart
     // tile length, so its samples stay the same bits (the svf scan, for one, depends on it)
     const size_t smem = render_smem_bytes(maxSlots, nOut, maxStateRows, maxParams, warpsPerCta, tileWidth, niterOverride);
     if (tileWidth == 1 && render_niter_for(1, niterOverride) == 4)
-        return launch_groups_impl<4, 0>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, stream);
+        return launch_groups_impl<4, 0>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, inOffset, stream);
     if (tileWidth == 2 && render_niter_for(2, niterOverride) == 8)
-        return launch_groups_impl<8, 1>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, stream);
+        return launch_groups_impl<8, 1>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, inOffset, stream);
     if (tileWidth == 32 && render_niter_for(32, niterOverride) == 4)
-        return launch_groups_impl<4, 5>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, stream);
+        return launch_groups_impl<4, 5>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, inOffset, stream);
     switch (tileWidth) {
-        case 32: return launch_groups_impl<8, 5>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, stream);
-        case 16: return launch_groups_impl<8, 4>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, stream);
-        case 8:  return launch_groups_impl<8, 3>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, stream);
-        case 4:  return launch_groups_impl<4, 2>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, stream);
-        case 2:  return launch_groups_impl<4, 1>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, stream);
-        default: return launch_groups_impl<1, 0>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, stream);
+        case 32: return launch_groups_impl<8, 5>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, inOffset, stream);
+        case 16: return launch_groups_impl<8, 4>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, inOffset, stream);
+        case 8:  return launch_groups_impl<8, 3>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, inOffset, stream);
+        case 4:  return launch_groups_impl<4, 2>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, inOffset, stream);
+        case 2:  return launch_groups_impl<4, 1>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, inOffset, stream);
+        default: return launch_groups_impl<1, 0>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, inOffset, stream);
     }
 }
 
 // One CTA of `stages` warps per one-voice graph (descs / tileStart are DEVICE pointers; the maxima size the per-graph shared memory).
 cudaError_t launch_render_groups_pipe(const LaunchParams* descs, const int* tileStart, int nGroups, int totalTiles, int stages,
-                                      int maxSlots, int nOut, int maxStateRows, int maxParams, long long sampleTime, int outOffset, cudaStream_t stream,
+                                      int maxSlots, int nOut, int maxStateRows, int maxParams, long long sampleTime, int outOffset, int inOffset, cudaStream_t stream,
                                       int niterOverride) {
     if (totalTiles <= 0) return cudaSuccess;
     if (stages < 1) stages = 1;
@@ -1199,18 +1202,18 @@ cudaError_t launch_render_groups_pipe(const LaunchParams* descs, const int* tile
     cudaError_t e = wide ? cudaFuncSetAttribute(render_groups_pipe_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem)
                          : cudaFuncSetAttribute(render_groups_pipe_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
     if (e != cudaSuccess) return e;
-    if (wide) render_groups_pipe_kernel<4><<<totalTiles, 32 * stages, smem, stream>>>(descs, tileStart, nGroups, totalTiles, (int) (graphBytes / sizeof(float)), sampleTime, outOffset);
-    else render_groups_pipe_kernel<1><<<totalTiles, 32 * stages, smem, stream>>>(descs, tileStart, nGroups, totalTiles, (int) (graphBytes / sizeof(float)), sampleTime, outOffset);
+    if (wide) render_groups_pipe_kernel<4><<<totalTiles, 32 * stages, smem, stream>>>(descs, tileStart, nGroups, totalTiles, (int) (graphBytes / sizeof(float)), sampleTime, outOffset, inOffset);
+    else render_groups_pipe_kernel<1><<<totalTiles, 32 * stages, smem, stream>>>(descs, tileStart, nGroups, totalTiles, (int) (graphBytes / sizeof(float)), sampleTime, outOffset, inOffset);
     return cudaGetLastError();
 }
 
-cudaError_t launch_mix_reduce(const float* partial, float* out, float* scratch, unsigned int* tickets, int nTiles, int nOut, int blockSize,
-                              int numSamples, cudaStream_t stream, HostDeliver hd) {
+cudaError_t launch_mix_reduce(const float* partial, float* out, int outStride, float* scratch, unsigned int* tickets, int nTiles, int nOut,
+                              int blockSize, int numSamples, cudaStream_t stream, HostDeliver hd) {
     const int chunksPerCh = (blockSize + 31) / 32;
     int G = (nTiles + 255) / 256;                 // ~8 tiles per lane per group; 4096 voices at L = 2 -> 8 groups x 16 chunks = 128 CTAs
     if (G > MIX_REDUCE_MAX_GROUPS) G = MIX_REDUCE_MAX_GROUPS;
     if (G < 1 || !scratch || !tickets) G = 1;
-    mix_reduce_kernel<<<dim3(nOut * chunksPerCh, G), 1024, 0, stream>>>(partial, out, scratch, tickets, nTiles, nOut, blockSize, numSamples, hd);
+    mix_reduce_kernel<<<dim3(nOut * chunksPerCh, G), 1024, 0, stream>>>(partial, out, scratch, tickets, nTiles, nOut, blockSize, outStride, numSamples, hd);
     return cudaGetLastError();
 }
 

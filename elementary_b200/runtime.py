@@ -71,6 +71,8 @@ def load_library() -> C.CDLL:
     lib.elem_b200_process_voices.argtypes = [C.c_void_p, _f32p, C.c_size_t, _f32p, _f32p, C.c_size_t, C.c_size_t]
     lib.elem_b200_render_offline.restype = C.c_int
     lib.elem_b200_render_offline.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, _f32p, C.c_size_t]
+    lib.elem_b200_process_offline.restype = C.c_int
+    lib.elem_b200_process_offline.argtypes = [C.c_void_p, _f32pp, C.c_size_t, _f32p, _f32pp, _f32p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p]
     lib.elem_b200_enqueue_block.restype = C.c_int
     lib.elem_b200_enqueue_block.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int]
     lib.elem_b200_peer_export.restype = C.c_int
@@ -270,6 +272,38 @@ class Runtime:
         assert out.flags["C_CONTIGUOUS"] and out.dtype == np.float32 and out.shape == (self.num_voices, num_outputs, n_blocks * self.block_size)
         self._check(self._lib.elem_b200_render_offline(self._h, num_outputs, n_blocks, out.ctypes.data_as(_f32p), chunk_blocks), "render_offline")
         return out
+
+    def process_offline(self, inputs: Optional[np.ndarray] = None, num_outputs: int = 1, num_samples: Optional[int] = None,
+                        voice_inputs: Optional[np.ndarray] = None, want_mix: bool = True, want_voices: bool = False,
+                        chunk_blocks: int = 0, sample_time: Optional[int] = None):
+        """OfflineRenderer.process (js/packages/offline-renderer/index.ts:87-133): ceil(n / block_size) full blocks in one call, with
+        ``inputs`` [n_in, n] broadcast to every voice or ``voice_inputs`` [voice, n_in, n] (zero past n), no host round trip per block.
+        ``num_samples`` defaults to the inputs' length (one block without inputs).  ``sample_time``: as for :meth:`process`, for the
+        first block.  Returns (mix [n_out, n] | None, voices [voice, n_out, n] | None), truncated to n."""
+        if inputs is not None and voice_inputs is not None:
+            raise ValueError("process_offline: give inputs or voice_inputs, not both")
+        src = inputs if inputs is not None else voice_inputs
+        keep = None if src is None else np.ascontiguousarray(np.asarray(src, dtype=np.float32))
+        n = int(num_samples if num_samples is not None else (keep.shape[-1] if keep is not None else self.block_size))
+        in_ptrs, vin_ptr, n_in = None, None, 0
+        if inputs is not None:
+            assert keep.ndim == 2 and keep.shape[1] == n
+            n_in = keep.shape[0]
+            if n_in:
+                in_ptrs = (_f32p * n_in)(*[keep[i].ctypes.data_as(_f32p) for i in range(n_in)])
+        elif voice_inputs is not None:
+            assert keep.ndim == 3 and keep.shape[0] == self.num_voices and keep.shape[2] == n
+            n_in = keep.shape[1]
+            vin_ptr = keep.ctypes.data_as(_f32p) if n_in else None
+        mix = np.zeros((num_outputs, n), dtype=np.float32) if want_mix else None
+        ov = np.zeros((self.num_voices, num_outputs, n), dtype=np.float32) if want_voices else None
+        mix_ptrs = (_f32p * max(1, num_outputs))(*[mix[i].ctypes.data_as(_f32p) for i in range(num_outputs)]) if want_mix else None
+        user = None if sample_time is None else C.byref(C.c_int64(int(sample_time)))
+        rc = self._lib.elem_b200_process_offline(self._h, in_ptrs, n_in, vin_ptr, mix_ptrs,
+                                                 ov.ctypes.data_as(_f32p) if ov is not None else None,
+                                                 num_outputs, n, int(chunk_blocks), user)
+        self._check(rc, "process_offline")
+        return mix, ov
 
     # -- device-resident stepping -----------------------------------------------------------------------------
     def enqueue_block(self, n_in: int = 0, n_out: int = 1, num_samples: Optional[int] = None, flags: int = FLAG_MIX) -> None:

@@ -31,7 +31,7 @@ extern "C" {
 
 typedef struct elem_b200_runtime elem_b200_runtime;
 
-/* Output channels of elem_b200_process / _process_voices / _enqueue_block (the mix bus past 8 channels is compact, see process). */
+/* Output channels of elem_b200_process / _process_voices / _enqueue_block / _process_offline (the mix bus past 8 channels is compact, see process). */
 #define ELEM_B200_MAX_OUT_CHANNELS 4096
 
 /* Runtime<float>::Runtime(double sampleRate, int blockSize)  — runtime/elem/Runtime.h:44,158-166.
@@ -109,8 +109,31 @@ int elem_b200_process_voices(elem_b200_runtime* rt, const float* in, size_t nIn,
 /* Offline rendering (what js/packages/offline-renderer does with process() in a loop; BASELINE config 5): numBlocks full blocks of every
  * voice, per-voice output hostOut[voice][nOut][numBlocks * blockSize] (host memory, nOut <= 8), no inputs, no mix bus.  Blocks are enqueued back to
  * back with no host synchronisation in between; outputs are written by the kernels into device chunk buffers of chunkBlocks blocks
- * (0 = default 32) and copied out on a second stream while the next chunk renders. */
+ * (0 = default 8; fewer when a chunk buffer would pass 256 MiB) and copied out on a second stream while the next chunk renders. */
 int elem_b200_render_offline(elem_b200_runtime* rt, size_t nOut, size_t numBlocks, float* hostOut, size_t chunkBlocks);
+
+/* OfflineRenderer.process(inputs, outputs) — js/packages/offline-renderer/index.ts:87-133: render a whole signal in one call, with inputs,
+ * through the chunk loop of elem_b200_render_offline (no host round trip per block).  All buffers are host memory.
+ *   in         nIn planar channels of numSamples, broadcast to every voice (as elem_b200_process), or NULL;
+ *   inVoices   per-voice inputs [voice][nIn][numSamples] (as elem_b200_process_voices), or NULL — not both with `in`;
+ *   mixOut     nOut planar channels of numSamples: the MIX BUS, or NULL;
+ *   voicesOut  per-voice outputs [voice][nOut][numSamples], or NULL.
+ * BLOCKS: ceil(numSamples / blockSize) FULL blocks, like the reference's offline renderer; input samples past numSamples are zero and the
+ *   outputs are truncated to numSamples.  A second call continues at the next block boundary.  numSamples == 0 renders nothing.
+ * BITS: block k of the mix is, bit for bit, what elem_b200_process returns for the same zero-padded block of inputs (the same summation
+ *   tree: K2 up to 8 channels, K2w past 8); per-voice outputs are those of elem_b200_process_voices.
+ * OUTPUT CHANNELS: the mix takes nOut <= 4096 (ELEM_B200_MAX_OUT_CHANNELS) with the channel rules of elem_b200_process (a channel no
+ *   running root aims at is +0.0); per-voice outputs nOut <= 8.  With voicesOut == NULL nothing per-voice is materialised or copied.
+ * SAMPLE CLOCK: userData NULL lets the engine clock run on; a pointer to an int64 t0 gives block k the time t0 + k * blockSize, as if
+ *   elem_b200_process had been called with that userData for each block.
+ * EVENTS are not polled inside the call: afterwards the event queues hold what as many elem_b200_process calls would have left.
+ * Blocks go through chunk buffers of chunkBlocks blocks (0 = default 8; fewer when a chunk buffer would pass 256 MiB): chunk k + 1's
+ *   inputs are uploaded and chunk k - 1's outputs copied out while chunk k renders.  The engine lock is held for the whole call.
+ * Returns -2, before rendering anything, when both `in` and `inVoices` are given, when nIn > 0 comes without an input pointer, when
+ *   nOut is 0 or above its limit, and with peers attached while the cross-GPU sum of process() is on ("process_allreduce" = 1): the
+ *   offline mix is not summed across GPUs. */
+int elem_b200_process_offline(elem_b200_runtime* rt, const float* const* in, size_t nIn, const float* inVoices,
+                              float* const* mixOut, float* voicesOut, size_t nOut, size_t numSamples, size_t chunkBlocks, void* userData);
 
 /* Device-resident stepping for throughput measurement and pipelines that keep audio in HBM: enqueue one block
  * on the engine's stream (no host copies, no synchronisation).  flags: 1 = read per-voice inputs from
