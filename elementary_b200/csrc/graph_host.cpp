@@ -70,6 +70,22 @@ cudaError_t Engine::dmemcpySync(void* dst, const void* src, size_t bytes, cudaMe
     if (e != cudaSuccess) return e;
     return cudaStreamSynchronize(stream_);
 }
+cudaError_t Engine::dzeroBlock(float* p, int pitch, size_t rows) {
+    if (planOnly_) { for (size_t r = 0; r < rows; ++r) std::memset(p + r * pitch, 0, sizeof(float) * blockSize_); return cudaSuccess; }
+    return cudaMemset2DAsync(p, sizeof(float) * pitch, 0, sizeof(float) * blockSize_, rows, stream_);
+}
+template <typename T> bool Engine::grow(T*& p, size_t& cap, size_t n, const char* what, bool zero, size_t slack, bool pinned) {
+    if (n <= cap) return true;
+    dsync();
+    if (pinned) { if (p) cudaFreeHost(p); }
+    else dfree(p);
+    p = nullptr; cap = 0;
+    const size_t bytes = sizeof(T) * n * slack;
+    if (!cuda(pinned ? cudaMallocHost((void**) &p, bytes) : dmalloc((void**) &p, bytes), what)) { p = nullptr; return false; }
+    if (zero && !cuda(pinned ? (std::memset(p, 0, bytes), cudaSuccess) : dmemset(p, 0, bytes), what)) return false;
+    cap = n * slack;
+    return true;
+}
 void Engine::dsync() { if (!planOnly_ && stream_) cudaStreamSynchronize(stream_); }
 void Engine::dsetdev() { if (!planOnly_) cudaSetDevice(device_); }
 void Engine::setStream(cudaStream_t s) {
@@ -160,27 +176,31 @@ Engine::Engine(double sampleRate, int blockSize, int numVoices, int device)
     auto g = std::make_unique<Group>();
     g->v0 = 0; g->nv = numVoices_; g->Vpad = (numVoices_ + 31) / 32 * 32;
     groups_.push_back(std::move(g));
-    mixFloats_ = (size_t) MAX_OUT_CHANNELS * blockSize_;
-    cuda(dmalloc((void**) &dMix_, sizeof(float) * MAX_OUT_CHANNELS * blockSize_), "cudaMalloc mix");
-    if (dMix_) cuda(dmemset(dMix_, 0, sizeof(float) * MAX_OUT_CHANNELS * blockSize_), "memset mix");
+    grow(dMix_, mixFloats_, (size_t) MAX_OUT_CHANNELS * blockSize_, "cudaMalloc mix", true);
     if (!planOnly_) {
         const size_t tick = (size_t) MAX_OUT_CHANNELS * ((blockSize_ + 31) / 32);
         cuda(cudaMalloc((void**) &dMixScratch_, sizeof(float) * MIX_REDUCE_MAX_GROUPS * MAX_OUT_CHANNELS * blockSize_), "cudaMalloc mix scratch");
         cuda(cudaMalloc((void**) &dMixTickets_, sizeof(unsigned int) * tick), "cudaMalloc mix tickets");
         if (dMixTickets_) cuda(cudaMemsetAsync(dMixTickets_, 0, sizeof(unsigned int) * tick, stream_), "memset mix tickets");
-        // mapped pinned mix bus + sequence word (HostDeliver); a failure here only disables the fast hand-over
-        const size_t mixFloats = (size_t) MAX_OUT_CHANNELS * blockSize_;
-        if (cudaHostAlloc((void**) &hMixHost_, sizeof(float) * mixFloats + 64, cudaHostAllocMapped) == cudaSuccess) {
-            std::memset(hMixHost_, 0, sizeof(float) * mixFloats + 64);
-            hMixFlag_ = reinterpret_cast<volatile uint32_t*>(hMixHost_ + mixFloats);
-            void* d = nullptr;
-            if (cudaHostGetDevicePointer(&d, hMixHost_, 0) == cudaSuccess && cudaMalloc((void**) &dDeliverDone_, sizeof(unsigned int)) == cudaSuccess) {
-                dMixHostAlias_ = static_cast<float*>(d);
-                dMixFlagAlias_ = reinterpret_cast<uint32_t*>(dMixHostAlias_ + mixFloats);
-                cudaMemsetAsync(dDeliverDone_, 0, sizeof(unsigned int), stream_);
-            } else { cudaFreeHost(hMixHost_); hMixHost_ = nullptr; hMixFlag_ = nullptr; }
-        } else { hMixHost_ = nullptr; cudaGetLastError(); }
+        // the fast hand-over of the mix bus (HostDeliver) needs both; a failure here only disables it
+        if (cudaMalloc((void**) &dDeliverDone_, sizeof(unsigned int)) == cudaSuccess) { cudaMemsetAsync(dDeliverDone_, 0, sizeof(unsigned int), stream_); allocMixHost(); }
+        else { dDeliverDone_ = nullptr; cudaGetLastError(); }
     }
+}
+
+// The mapped pinned copy of the mix bus, mixFloats_ floats, and the sequence word behind it (HostDeliver).  A failure only disables the
+// fast hand-over: hMixHost_ stays null.
+void Engine::allocMixHost() {
+    if (hMixHost_) cudaFreeHost(hMixHost_);
+    hMixHost_ = nullptr; hMixFlag_ = nullptr; dMixHostAlias_ = nullptr; dMixFlagAlias_ = nullptr;
+    const size_t bytes = sizeof(float) * mixFloats_ + 64;
+    void* d = nullptr;
+    if (cudaHostAlloc((void**) &hMixHost_, bytes, cudaHostAllocMapped) != cudaSuccess) { hMixHost_ = nullptr; cudaGetLastError(); return; }
+    if (cudaHostGetDevicePointer(&d, hMixHost_, 0) != cudaSuccess) { cudaFreeHost(hMixHost_); hMixHost_ = nullptr; cudaGetLastError(); return; }
+    std::memset(hMixHost_, 0, bytes);
+    hMixFlag_ = reinterpret_cast<volatile uint32_t*>(hMixHost_ + mixFloats_);
+    dMixHostAlias_ = static_cast<float*>(d);
+    dMixFlagAlias_ = reinterpret_cast<uint32_t*>(dMixHostAlias_ + mixFloats_);
 }
 
 static void freeGroupStorage(Group& g, bool plan) {
@@ -220,8 +240,8 @@ Engine::~Engine() {
     if (dWideTickets_) dfree(dWideTickets_);
     if (dOutCompact_) dfree(dOutCompact_);
     for (auto& kv : batch_) { if (kv.second.dDescs) dfree(kv.second.dDescs); if (kv.second.dTileStart) dfree(kv.second.dTileStart); }
-    for (auto* l : {&timedEvents_, &timedMixEvents_, &timedConvEvents_, &timedXchgEvents_})
-        for (auto& ev : *l) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
+    for (auto& l : timed_)
+        for (auto& ev : l) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
     for (auto& ev : eventPool_) { cudaEventDestroy(ev.first); cudaEventDestroy(ev.second); }
     if (ownStream_ && stream_) cudaStreamDestroy(stream_);
 }
@@ -2269,90 +2289,14 @@ int Engine::compile(Group& g, int nIn, std::shared_ptr<Program>& out) {
 
 // ---------------------------------------------------------------------------------------------------------
 // process
-int Engine::ensureBuffers(size_t nIn, size_t nOut, bool perVoiceIn, bool materialise, size_t wideRows, size_t wideOutRows) {
-    size_t tiles = 0;
-    for (auto& g : groups_) tiles += (size_t) g->nTiles();
-    const bool wide = nOut > (size_t) MAX_OUT_CHANNELS;
-    const size_t pf = wide ? std::max<size_t>(1, wideRows) * blockSize_ : std::max<size_t>(1, tiles) * nOut * blockSize_;
-    if (pf > partialFloats_) {
-        dsync();
-        if (dPartial_) dfree(dPartial_);
-        if (!cuda(dmalloc((void**) &dPartial_, sizeof(float) * pf), "cudaMalloc partial")) return rc::CudaError;
-        dmemset(dPartial_, 0, sizeof(float) * pf);
-        partialFloats_ = pf;
-    }
-    if (materialise && !offlineOut_) {
-        const size_t of = (size_t) numVoices_ * nOut * blockSize_;
-        if (of > outVoiceFloats_) {
-            dsync();
-            if (dOutVoice_) dfree(dOutVoice_);
-            if (!cuda(dmalloc((void**) &dOutVoice_, sizeof(float) * of), "cudaMalloc voice out")) return rc::CudaError;
-            outVoiceFloats_ = of;
-            wide_.outZeroValid = false;
-        }
-        const size_t cf = wide ? std::max<size_t>(1, wideOutRows) * blockSize_ : 0;
-        if (cf > outCompactFloats_) {
-            dsync();
-            if (dOutCompact_) dfree(dOutCompact_);
-            if (!cuda(dmalloc((void**) &dOutCompact_, sizeof(float) * cf), "cudaMalloc compact voice out")) { dOutCompact_ = nullptr; outCompactFloats_ = 0; return rc::CudaError; }
-            outCompactFloats_ = cf;
-        }
-    }
-    // the mix bus and its mapped host copy grow to the widest nOut used (elem_b200_mix_device: the pointer moves then)
-    const size_t mf = nOut * blockSize_;
-    if (mf > mixFloats_) {
-        dsync();
-        if (dMix_) dfree(dMix_);
-        dMix_ = nullptr; mixFloats_ = 0;
-        if (!cuda(dmalloc((void**) &dMix_, sizeof(float) * mf), "cudaMalloc mix")) return rc::CudaError;
-        dmemset(dMix_, 0, sizeof(float) * mf);
-        mixFloats_ = mf;
-        if (hMixHost_) {   // a failure here only disables the fast hand-over, as at construction
-            cudaFreeHost(hMixHost_);
-            hMixHost_ = nullptr; hMixFlag_ = nullptr; dMixHostAlias_ = nullptr; dMixFlagAlias_ = nullptr;
-            void* d = nullptr;
-            if (cudaHostAlloc((void**) &hMixHost_, sizeof(float) * mf + 64, cudaHostAllocMapped) == cudaSuccess) {
-                std::memset(hMixHost_, 0, sizeof(float) * mf + 64);
-                if (cudaHostGetDevicePointer(&d, hMixHost_, 0) == cudaSuccess) {
-                    hMixFlag_ = reinterpret_cast<volatile uint32_t*>(hMixHost_ + mf);
-                    dMixHostAlias_ = static_cast<float*>(d);
-                    dMixFlagAlias_ = reinterpret_cast<uint32_t*>(dMixHostAlias_ + mf);
-                } else { cudaFreeHost(hMixHost_); hMixHost_ = nullptr; cudaGetLastError(); }
-            } else { hMixHost_ = nullptr; cudaGetLastError(); }
-        }
-    }
-    if (offlineIn_) return rc::Ok;   // the inputs are in an offline chunk
-    if (perVoiceIn && nIn) { if (!voiceInDevicePtr(nIn)) return rc::CudaError; }
-    else if (nIn) { if (!sharedInDevicePtr(nIn)) return rc::CudaError; }
-    return rc::Ok;
-}
-
 float* Engine::voiceInDevicePtr(size_t nIn) {
     Lock lk(mu_);
-    const size_t f = (size_t) numVoices_ * nIn * blockSize_;
-    if (f > inVoiceFloats_) {
-        dsync();
-        if (dInVoice_) dfree(dInVoice_);
-        dInVoice_ = nullptr;
-        if (!cuda(dmalloc((void**) &dInVoice_, sizeof(float) * f), "cudaMalloc voice in")) return nullptr;
-        dmemset(dInVoice_, 0, sizeof(float) * f);
-        inVoiceFloats_ = f;
-    }
-    return dInVoice_;
+    return grow(dInVoice_, inVoiceFloats_, (size_t) numVoices_ * nIn * blockSize_, "cudaMalloc voice in", true) ? dInVoice_ : nullptr;
 }
 
 float* Engine::sharedInDevicePtr(size_t nIn) {
     Lock lk(mu_);
-    const size_t f = nIn * blockSize_;
-    if (f > inSharedFloats_) {
-        dsync();
-        if (dInShared_) dfree(dInShared_);
-        dInShared_ = nullptr;
-        if (!cuda(dmalloc((void**) &dInShared_, sizeof(float) * f), "cudaMalloc shared in")) return nullptr;
-        dmemset(dInShared_, 0, sizeof(float) * f);
-        inSharedFloats_ = f;
-    }
-    return dInShared_;
+    return grow(dInShared_, inSharedFloats_, nIn * blockSize_, "cudaMalloc shared in", true) ? dInShared_ : nullptr;
 }
 
 int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoiceIn, bool materialise, bool mix, bool allReduce) {
@@ -2360,49 +2304,90 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
     // A plan-only engine cannot render.  With option "plan_dry_run" it still walks the whole host side of a block — program swap,
     // recompiles, descriptors, fades, event mirrors — and skips exactly the CUDA calls: the thread-safety tests (TSAN, no GPU) use it.
     if (planOnly_ && !planDryRun_) return fail(rc::CudaError, "plan-only runtime (no CUDA device): rendering is impossible, there is no CPU fallback");
-    const bool dry = planOnly_;
     dsetdev();
     if (numSamples > (size_t) blockSize_ || nOut > (size_t) MAX_WIDE_OUT_CHANNELS) return fail(rc::BadArgument, "numSamples > blockSize or too many output channels");
+    if (nOut > (size_t) MAX_OUT_CHANNELS && mix && allReduce && peerAttached_ && peer_.world > 1)
+        return fail(rc::BadArgument, "the cross-GPU mix bus carries at most 8 output channels (its exchange buffer is sized at export)");
+    BlockIO io;
+    io.nIn = nIn; io.nOut = nOut; io.numSamples = numSamples; io.perVoiceIn = perVoiceIn; io.allReduce = allReduce;
+    io.inPitch = io.outPitch = io.mixPitch = blockSize_;
+    // input rows the caller never wrote read as zero
+    if (nIn && !(io.in = perVoiceIn ? voiceInDevicePtr(nIn) : sharedInDevicePtr(nIn))) return rc::CudaError;
+    if (materialise) {
+        const size_t of = (size_t) numVoices_ * nOut * blockSize_;
+        // K1 writes [voice][nOut] in the dense layout, and new memory is not cleared: the wide path clears the buffer again
+        if (nOut <= (size_t) MAX_OUT_CHANNELS || of > outVoiceFloats_) wide_.outZeroValid = false;
+        if (!grow(dOutVoice_, outVoiceFloats_, of, "cudaMalloc voice out")) return rc::CudaError;
+        io.voiceOut = dOutVoice_;
+    }
+    // the mix bus and its mapped host copy grow to the widest nOut used (elem_b200_mix_device: the pointer moves then)
+    if (nOut * blockSize_ > mixFloats_) {
+        if (!grow(dMix_, mixFloats_, nOut * blockSize_, "cudaMalloc mix", true)) return rc::CudaError;
+        if (hMixHost_) allocMixHost();
+    }
+    if (mix) io.mix = dMix_;
+    return enqueueBlock(io);
+}
+
+// One block (the engine lock is held): the walk over the voice groups unless the steady-state key matches, then the launches every
+// block ends with — the many-groups buckets, the mix bus (K2, K2w or silence) and the cross-GPU sum (K4).
+int Engine::enqueueBlock(const BlockIO& io) {
+    const bool dry = planOnly_;
+    const size_t nOut = io.nOut, numSamples = io.numSamples;
     // Past MAX_OUT_CHANNELS the mix bus is compact (DESIGN.md section 3): per channel, only the partial rows of the groups that aim at it
     const bool wide = nOut > (size_t) MAX_OUT_CHANNELS;
-    if (wide && mix && allReduce && peerAttached_ && peer_.world > 1)
-        return fail(rc::BadArgument, "the cross-GPU mix bus carries at most 8 output channels (its exchange buffer is sized at export)");
-    if (wide && offlineOut_) return fail(rc::BadArgument, "renderOffline: at most 8 output channels");
-    if (!wide && materialise && !offlineOut_) wide_.outZeroValid = false;   // K1 writes [voice][nOut] in the dense layout
-
-    // the cached descriptors hold the I/O base pointers: any change of where inputs or outputs live (an offline chunk slot) is a new key
-    const size_t key[7] = {nIn, nOut, numSamples, (size_t) perVoiceIn, (size_t) materialise | ((size_t) (uintptr_t) offlineOut_ << 1),
-                           (size_t) mix | ((size_t) offlineStride_ << 1), (size_t) (uintptr_t) offlineIn_};
-    // an offline block reads its inputs from column offlineOffset_ of the input chunk and leaves its mix in the same column of the mix chunk
-    const int inStride = offlineIn_ ? offlineStride_ : blockSize_, inOffset = offlineIn_ ? offlineOffset_ : 0;
-    const int outOffset = offlineOut_ ? offlineOffset_ : 0;
-    float* const mixDst = offlineMix_ ? offlineMix_ + offlineOffset_ : dMix_;
-    const int mixStride = offlineMix_ ? offlineStride_ : blockSize_;
-    if (steadyValid_ && !dry && std::memcmp(key, steadyKey_, sizeof key) == 0) {
-        for (auto& sb : steadyBuckets_) {
-            BatchBuffers& bb = batch_[sb.key];
-            auto ev = timedBegin();
-            if (!cuda(sb.pipeStages >= 1
-                          ? launch_render_groups_pipe(bb.dDescs, bb.dTileStart, sb.nGroups, sb.totalTiles, sb.pipeStages, sb.maxSlots, sb.smemOut, sb.maxState, sb.maxParams, sampleTime_, outOffset, inOffset, stream_, opt_.niter)
-                          : launch_render_groups(bb.dDescs, bb.dTileStart, sb.nGroups, sb.totalTiles, sb.L, sb.maxSlots, sb.smemOut, sb.maxState, sb.maxParams, sb.wpc, sampleTime_, outOffset, inOffset, stream_, opt_.niter),
-                      "render groups kernel launch")) return rc::CudaError;
-            if (timeKernels_) { cudaEventRecord(ev.second, stream_); timedEvents_.push_back(ev); }
-            ++launches_;
-        }
-        if (wide) {
-            const int rw = launchWide(nOut, numSamples, materialise, mix);
-            if (rw != rc::Ok) return rw;
-        } else if (mix) {
-            auto ev = timedBegin();
-            if (!cuda(launch_mix_reduce(dPartial_, mixDst, mixStride, dMixScratch_, dMixTickets_, steadyTiles_, (int) nOut, blockSize_, (int) numSamples, stream_, takeDeliver()), "mix reduce launch")) return rc::CudaError;
-            if (timeKernels_) { cudaEventRecord(ev.second, stream_); timedMixEvents_.push_back(ev); }
-            ++launches_;
-        }
-        curNOut_ = nOut;
-        sampleTime_ += (int64_t) numSamples;
-        return rc::Ok;
+    // the scatter to [voice][nOut] writes the engine's own buffer at pitch blockSize
+    if (wide && io.voiceOut && io.voiceOut != dOutVoice_) return fail(rc::BadArgument, "renderOffline: at most 8 output channels");
+    if (!steadyValid_ || !io.sameSteadyKey(steadyIO_)) {
+        const int r = walkGroups(io);
+        if (r != rc::Ok) return r;
     }
-    bool allSteady = !(allReduce && peerAttached_ && peer_.world > 1), allBatched = true;
+    for (auto& sb : steadyBuckets_) {
+        BatchBuffers& bb = batch_[sb.key];
+        auto ev = timedBegin();
+        if (!dry && !cuda(sb.pipeStages >= 1
+                              ? launch_render_groups_pipe(bb.dDescs, bb.dTileStart, sb.nGroups, sb.totalTiles, sb.pipeStages, sb.maxSlots, sb.smemOut, sb.maxState, sb.maxParams, sampleTime_, io.col, io.col, stream_, opt_.niter)
+                              : launch_render_groups(bb.dDescs, bb.dTileStart, sb.nGroups, sb.totalTiles, sb.L, sb.maxSlots, sb.smemOut, sb.maxState, sb.maxParams, sb.wpc, sampleTime_, io.col, io.col, stream_, opt_.niter),
+                  "render groups kernel launch")) return rc::CudaError;
+        timedEnd(ev, 0);
+        ++launches_;
+    }
+    // With the cross-GPU sum behind it, K2 leaves this rank's partial mix in PeerMix::own (K4 pushes it to the peers from there and
+    // writes the total to the mix bus): no staging copy, no in-place hazard between K4's CTAs.
+    const bool exchange = io.mix && io.allReduce && peerAttached_ && peer_.world > 1;
+    if (exchange) ++peerEpoch_;
+    if (wide) {
+        const int rw = dry ? rc::Ok : launchWide(io);
+        if (rw != rc::Ok) return rw;
+    } else if (io.mix) {
+        float* const mixOut = exchange ? peer_.own : io.mix + io.col;
+        const int pitch = exchange ? blockSize_ : io.mixPitch;
+        if (steadyTiles_ > 0) {
+            auto ev = timedBegin();
+            if (!dry && !cuda(launch_mix_reduce(dPartial_, mixOut, pitch, dMixScratch_, dMixTickets_, steadyTiles_, (int) nOut, blockSize_, (int) numSamples, stream_, exchange ? HostDeliver{} : takeDeliver()), "mix reduce launch")) return rc::CudaError;
+            timedEnd(ev, 1);
+            ++launches_;
+        } else if (!cuda(dzeroBlock(mixOut, pitch, nOut), "memset mix")) return rc::CudaError;   // an offline chunk's slots are reused: every block writes its column
+    }
+    if (exchange) {   // K4: the cross-GPU sum of the mix bus, in the same stream
+        auto ev = timedBegin();
+        if (!cuda(launch_mix_exchange(peer_, dMix_, (int) (nOut * blockSize_), peerEpoch_, dPeerStatus_, stream_, takeDeliver()), "mix exchange launch")) return rc::CudaError;
+        timedEnd(ev, 3);
+        ++launches_;
+    }
+    sampleTime_ += (int64_t) numSamples;   // wasm/Main.cpp:217
+    return rc::Ok;
+}
+
+// The slow walk of a block: program swaps and recompiles, the wide plan, buffers, the launches of voice groups that run on their own (K1 /
+// K3), fades and event mirrors, and the many-groups buckets (steadyBuckets_) with their descriptors uploaded when they changed.
+int Engine::walkGroups(const BlockIO& io) {
+    const bool dry = planOnly_;
+    const size_t nIn = io.nIn, nOut = io.nOut, numSamples = io.numSamples;
+    const bool perVoiceIn = io.perVoiceIn, materialise = io.voiceOut != nullptr, mix = io.mix != nullptr;
+    const bool wide = nOut > (size_t) MAX_OUT_CHANNELS;
+    steadyValid_ = false;
+    bool allSteady = !(io.allReduce && peerAttached_ && peer_.world > 1), allBatched = true;
 
     // Runtime::process: swap in the newest render sequence (Runtime.h:277-285); recompile when the number of
     // host input channels a leaf node sees has changed.
@@ -2476,11 +2461,14 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
                     for (int c : wideCh[gi]) w.dstRow.push_back((g.v0 + v) * (int) nOut + c);
             }
     }
-    int r = ensureBuffers(nIn, nOut, perVoiceIn, materialise, wideRows, wideOutRows);
-    if (r != rc::Ok) return r;
-    const float* const inBase = offlineIn_ ? offlineIn_ : (perVoiceIn ? dInVoice_ : dInShared_);   // (ensureBuffers may have moved these)
+    size_t tiles = 0;
+    for (auto& g : groups_) tiles += (size_t) g->nTiles();
+    if (!grow(dPartial_, partialFloats_, wide ? std::max<size_t>(1, wideRows) * blockSize_ : std::max<size_t>(1, tiles) * nOut * blockSize_, "cudaMalloc partial", true))
+        return rc::CudaError;
+    if (materialise && wide && !grow(dOutCompact_, outCompactFloats_, std::max<size_t>(1, wideOutRows) * blockSize_, "cudaMalloc compact voice out"))
+        return rc::CudaError;
     if (wide && !dry) {
-        r = uploadWidePlan();
+        const int r = uploadWidePlan();
         if (r != rc::Ok) return r;
     }
 
@@ -2490,12 +2478,12 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
         Group& g = *gp;
         const size_t gi = (size_t) (&gp - groups_.data());
         const int nTiles = g.nTiles();
-        if (!g.active || nTiles == 0) { allSteady = false; }
         if (!g.active || nTiles == 0) {
+            allSteady = false;
             // no render sequence yet: outputs are silence (Runtime.h:287-289 leaves the host buffers untouched;
             // we define the voice's contribution as zero)
             if (nTiles && mix && !wide) dmemset(dPartial_ + (size_t) tileBase * nOut * blockSize_, 0, sizeof(float) * (size_t) nTiles * nOut * blockSize_);
-            if (materialise && dOutVoice_ && !offlineOut_) dmemset(dOutVoice_ + (size_t) g.v0 * nOut * blockSize_, 0, sizeof(float) * (size_t) g.nv * nOut * blockSize_);
+            if (materialise) dzeroBlock(io.voiceOut + (size_t) g.v0 * nOut * io.outPitch + io.col, io.outPitch, (size_t) g.nv * nOut);
             tileBase += nTiles;
             continue;
         }
@@ -2508,12 +2496,12 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
         P.rows = g.dRows;
         // wide: the group's own runs of compact rows, per-voice I/O indexed from its first voice (voice0 = 0)
         const std::vector<int>* const gch = wide ? &wideCh[gi] : nullptr;
-        float* const voiceOut = wide ? (gch->empty() ? nullptr : dOutCompact_ + wideOutBase[gi] * blockSize_) : (offlineOut_ ? offlineOut_ : dOutVoice_);
+        float* const voiceOut = wide ? (gch->empty() ? nullptr : dOutCompact_ + wideOutBase[gi] * blockSize_) : io.voiceOut;
         float* const partialOut = wide ? (gch->empty() ? nullptr : dPartial_ + wideRowBase[gi] * blockSize_) : dPartial_;
-        // input rows without this block's column offset (the many-groups launches take it as an argument; single-group launches are
-        // handed pointers that include it)
-        const float* const inShared = (!perVoiceIn && nIn) ? inBase : nullptr;
-        const float* const inVoice = (perVoiceIn && nIn) ? inBase + (wide ? (size_t) g.v0 * nIn * inStride : 0) : nullptr;
+        // input rows without this block's column (the many-groups launches take it as an argument; single-group launches are handed
+        // pointers that include it)
+        const float* const inShared = (!perVoiceIn && nIn) ? io.in : nullptr;
+        const float* const inVoice = (perVoiceIn && nIn) ? io.in + (wide ? (size_t) g.v0 * nIn * io.inPitch : 0) : nullptr;
         P.inShared = inShared;
         P.inVoice = inVoice;
         P.outVoice = materialise ? voiceOut : nullptr;
@@ -2529,8 +2517,8 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
         P.blockSize = blockSize_;
         P.nIn = (int) nIn;
         P.nOut = wide ? (int) gch->size() : (int) nOut;
-        P.inStride = inStride;
-        P.outStride = offlineOut_ ? offlineStride_ : blockSize_;
+        P.inStride = io.inPitch;
+        P.outStride = io.outPitch;
         P.tileBase = wide ? 0 : tileBase;
         uint32_t runMask = 0;
         for (size_t ri = 0; ri < p.rootIds.size(); ++ri) {
@@ -2602,16 +2590,11 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
             allBatched = false;
             const bool last = stg + 1 == nStages;
             P.code = p.dCode + (p.stages.empty() ? 0 : p.stages[stg].codeOffset);
-            P.outVoice = (last && materialise) ? voiceOut + outOffset : nullptr;   // outputs and taps belong to the last stage
-            P.inShared = inShared ? inShared + inOffset : nullptr;
-            P.inVoice = inVoice ? inVoice + inOffset : nullptr;
+            P.outVoice = (last && materialise) ? voiceOut + io.col : nullptr;   // outputs and taps belong to the last stage
+            P.inShared = inShared ? inShared + io.col : nullptr;
+            P.inVoice = inVoice ? inVoice + io.col : nullptr;
             P.mixPartial = (last && mix) ? partialOut : nullptr;
-            std::pair<cudaEvent_t, cudaEvent_t> ev{nullptr, nullptr};
-            if (timeKernels_) {
-                if (!eventPool_.empty()) { ev = eventPool_.back(); eventPool_.pop_back(); }
-                else { cudaEventCreate(&ev.first); cudaEventCreate(&ev.second); }
-                cudaEventRecord(ev.first, stream_);
-            }
+            auto ev = timedBegin();
             const bool emptyStage = !p.stages.empty() && ((p.stages[stg].empty && !last) || (last && p.fusedConvStage >= 0));   // fused: K3's epilogue did the root
             if (!emptyStage) {
                 const SpecKernel* spec = nullptr;
@@ -2624,7 +2607,7 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
                 if (!dry && !cuda(launch_render_block(P, wpc, opt_.niter, stream_, spec), "render kernel launch")) return rc::CudaError;
                 ++launches_;
             }
-            if (timeKernels_) { cudaEventRecord(ev.second, stream_); timedEvents_.push_back(ev); }
+            timedEnd(ev, 0);   // recorded around a skipped stage too
             if (p.stages.empty()) continue;
             // K3: the convolvers fed by this stage (ConvolutionNode::process, wasm/Convolve.h:58-85); a call longer
             // than what is left of the current 512-sample partition is cut like FFTConvolver.cpp:155-203 does
@@ -2641,28 +2624,23 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
                     epi.gain0 = rd.gain0; epi.step = rd.step; epi.target = rd.target; epi.channel = rd.channel;
                     epi.nOut = P.nOut; epi.blockSize = blockSize_;
                     epi.mixPartial = mix ? partialOut : nullptr; epi.tileBase = P.tileBase;
-                    epi.outVoice = materialise ? voiceOut + outOffset : nullptr;
+                    epi.outVoice = materialise ? voiceOut + io.col : nullptr;
                     epi.voice0 = P.voice0; epi.outStride = P.outStride; epi.outOffset = 0;
                 }
                 int offset = 0;
                 while (offset < (int) numSamples) {
                     const int n = cs.maxS == 0 ? (int) numSamples - offset
                                                      : std::min((int) numSamples - offset, CONV_BLOCK - cs.fill);
-                    std::pair<cudaEvent_t, cudaEvent_t> ev3{nullptr, nullptr};
-                    if (timeKernels_) {
-                        if (!eventPool_.empty()) { ev3 = eventPool_.back(); eventPool_.pop_back(); }
-                        else { cudaEventCreate(&ev3.first); cudaEventCreate(&ev3.second); }
-                        cudaEventRecord(ev3.first, stream_);
-                    }
+                    auto ev3 = timedBegin();
                     const float* cin = cv.in;
                     int cinStride = blockSize_;
-                    if (cv.inChannel >= 0) {   // straight from the host input buffers: per-voice [voice][nIn][inStride] or shared [nIn][inStride]
-                        if (perVoiceIn) { cin = inBase + ((size_t) g.v0 * nIn + cv.inChannel) * inStride + inOffset; cinStride = (int) nIn * inStride; }
-                        else { cin = inBase + (size_t) cv.inChannel * inStride + inOffset; cinStride = 0; }
+                    if (cv.inChannel >= 0) {   // straight from the host input rows: per-voice [voice][nIn][inPitch] or shared [nIn][inPitch]
+                        if (perVoiceIn) { cin = io.in + ((size_t) g.v0 * nIn + cv.inChannel) * io.inPitch + io.col; cinStride = (int) nIn * io.inPitch; }
+                        else { cin = io.in + (size_t) cv.inChannel * io.inPitch + io.col; cinStride = 0; }
                     }
                     if (!dry && !cuda(convolver_process_chunk(cs, cin, cinStride, cv.out, blockSize_, offset, n, stream_, epi), "convolver launch")) return rc::CudaError;
                     if (dry) { offset += n; continue; }
-                    if (timeKernels_) { cudaEventRecord(ev3.second, stream_); timedConvEvents_.push_back(ev3); }
+                    timedEnd(ev3, 2);
                     ++launches_;
                     offset += n;
                 }
@@ -2694,15 +2672,9 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
         // descriptors change only while roots fade or when graphs change: re-upload only then
         BatchBuffers& bb = batch_[kv.first];
         const size_t dbytes = descs.size() * sizeof(LaunchParams), tbytes = tileStart.size() * sizeof(int);
-        if (bb.capGroups < descs.size()) {
-            dsync();
-            if (bb.dDescs) dfree(bb.dDescs);
-            if (bb.dTileStart) dfree(bb.dTileStart);
-            bb.capGroups = descs.size() * 2;
-            if (!cuda(dmalloc((void**) &bb.dDescs, bb.capGroups * sizeof(LaunchParams)), "cudaMalloc group descriptors")) return rc::CudaError;
-            if (!cuda(dmalloc((void**) &bb.dTileStart, bb.capGroups * sizeof(int)), "cudaMalloc tile table")) return rc::CudaError;
-            bb.lastDescs.clear();
-        }
+        if (descs.size() > bb.capDescs) bb.lastDescs.clear();
+        if (!grow(bb.dDescs, bb.capDescs, descs.size(), "cudaMalloc group descriptors", false, 2) ||
+            !grow(bb.dTileStart, bb.capTiles, descs.size(), "cudaMalloc tile table", false, 2)) return rc::CudaError;
         if (!dry && (bb.lastDescs.size() != dbytes || std::memcmp(bb.lastDescs.data(), descs.data(), dbytes) != 0)) {
             if (!cuda(cudaMemcpyAsync(bb.dDescs, descs.data(), dbytes, cudaMemcpyHostToDevice, stream_), "upload group descriptors")) return rc::CudaError;
             if (!cuda(cudaMemcpyAsync(bb.dTileStart, tileStart.data(), tbytes, cudaMemcpyHostToDevice, stream_), "upload tile table")) return rc::CudaError;
@@ -2711,56 +2683,11 @@ int Engine::enqueueBlock(size_t nIn, size_t nOut, size_t numSamples, bool perVoi
         int wpc = opt_.warpsPerCta;
         if (wpc <= 0) wpc = total >= smCount_ * 8 ? 4 : (total >= smCount_ * 4 ? 2 : 1);
         while (wpc > 1 && render_smem_bytes(maxSlots, smemOut, maxState, maxParams, wpc, L, opt_.niter) > 200 * 1024) wpc >>= 1;
-        std::pair<cudaEvent_t, cudaEvent_t> ev{nullptr, nullptr};
-        if (timeKernels_) {
-            if (!eventPool_.empty()) { ev = eventPool_.back(); eventPool_.pop_back(); }
-            else { cudaEventCreate(&ev.first); cudaEventCreate(&ev.second); }
-            cudaEventRecord(ev.first, stream_);
-        }
         steadyBuckets_.push_back(SteadyBucket{L, (int) descs.size(), total, maxSlots, maxState, maxParams, wpc, pipeStages, kv.first, smemOut});
-        if (!dry && !cuda(pipeStages >= 1
-                              ? launch_render_groups_pipe(bb.dDescs, bb.dTileStart, (int) descs.size(), total, pipeStages, maxSlots, smemOut, maxState, maxParams, sampleTime_, outOffset, inOffset, stream_, opt_.niter)
-                              : launch_render_groups(bb.dDescs, bb.dTileStart, (int) descs.size(), total, L, maxSlots, smemOut, maxState, maxParams, wpc, sampleTime_, outOffset, inOffset, stream_, opt_.niter),
-                  "render groups kernel launch")) return rc::CudaError;
-        if (timeKernels_) { cudaEventRecord(ev.second, stream_); timedEvents_.push_back(ev); }
-        ++launches_;
-    }
-    // With the cross-GPU sum behind it, K2 leaves this rank's partial mix in PeerMix::own (K4 pushes it to the peers from there and
-    // writes the total to the mix bus): no staging copy, no in-place hazard between K4's CTAs.
-    const bool exchange = mix && allReduce && peerAttached_ && peer_.world > 1;
-    float* mixOut = mixDst;
-    if (exchange) {
-        ++peerEpoch_;
-        mixOut = peer_.own;
-    }
-    if (wide) {
-        if (!dry) {
-            const int rw = launchWide(nOut, numSamples, materialise, mix);
-            if (rw != rc::Ok) return rw;
-        }
-    } else if (mix) {
-        if (tileBase > 0) {
-            auto ev = timedBegin();
-            if (!dry && !cuda(launch_mix_reduce(dPartial_, mixOut, exchange ? blockSize_ : mixStride, dMixScratch_, dMixTickets_, tileBase, (int) nOut, blockSize_, (int) numSamples, stream_, exchange ? HostDeliver{} : takeDeliver()), "mix reduce launch")) return rc::CudaError;
-            if (timeKernels_) { cudaEventRecord(ev.second, stream_); timedMixEvents_.push_back(ev); }
-            ++launches_;
-        } else if (offlineMix_) {   // the chunk's slots are reused: this block's column of every row is written on every block
-            if (!dry && !cuda(cudaMemset2DAsync(mixDst, sizeof(float) * mixStride, 0, sizeof(float) * blockSize_, nOut, stream_), "memset offline mix")) return rc::CudaError;
-        } else {
-            dmemset(mixOut, 0, sizeof(float) * nOut * blockSize_);
-        }
-    }
-    if (exchange) {   // K4: the cross-GPU sum of the mix bus, in the same stream
-        auto ev = timedBegin();
-        if (!cuda(launch_mix_exchange(peer_, dMix_, (int) (nOut * blockSize_), peerEpoch_, dPeerStatus_, stream_, takeDeliver()), "mix exchange launch")) return rc::CudaError;
-        if (timeKernels_) { cudaEventRecord(ev.second, stream_); timedXchgEvents_.push_back(ev); }
-        ++launches_;
     }
     steadyValid_ = allSteady && allBatched && !buckets.empty() && !dry;
-    std::memcpy(steadyKey_, key, sizeof key);
+    steadyIO_ = io;
     steadyTiles_ = tileBase;
-    curNOut_ = nOut;
-    sampleTime_ += (int64_t) numSamples;   // wasm/Main.cpp:217
     return rc::Ok;
 }
 
@@ -2783,13 +2710,8 @@ int Engine::uploadWidePlan() {
     auto upload = [&](auto& dev, size_t& cap, const auto& host, auto& shadow, const char* what) -> bool {
         typedef typename std::remove_reference<decltype(host)>::type::value_type T;
         const size_t n = std::max<size_t>(1, host.size());
-        if (n > cap) {
-            dsync();
-            if (dev) dfree(dev);
-            dev = nullptr; cap = 0; shadow.clear();
-            if (!cuda(dmalloc((void**) &dev, n * 2 * sizeof(T)), what)) { dev = nullptr; return false; }
-            cap = n * 2;
-        }
+        if (n > cap) shadow.clear();
+        if (!grow(dev, cap, n, what, false, 2)) return false;
         const size_t bytes = host.size() * sizeof(T);
         if (shadow.size() == bytes / sizeof(shadow[0]) && std::memcmp(shadow.data(), host.data(), bytes) == 0) return true;
         if (bytes && !cuda(dmemcpy(dev, host.data(), bytes, cudaMemcpyHostToDevice), what)) return false;
@@ -2800,25 +2722,18 @@ int Engine::uploadWidePlan() {
     if (!upload(w.dRows, w.capRows, w.rows, w.upRows, "upload wide row lists")) return rc::CudaError;
     if (!upload(w.dSegs, w.capSegs, w.segs, w.upSegs, "upload wide segments")) return rc::CudaError;
     if (!upload(w.dDst, w.capDst, w.dstRow, w.upDst, "upload wide output rows")) return rc::CudaError;
-    if ((size_t) w.nScratch > wideScratchRows_) {
-        dsync();
-        if (dWideScratch_) dfree(dWideScratch_);
-        if (dWideTickets_) dfree(dWideTickets_);
-        dWideScratch_ = nullptr; dWideTickets_ = nullptr; wideScratchRows_ = 0;
-        const size_t rowsCap = (size_t) w.nScratch * 2, tick = rowsCap * ((blockSize_ + 31) / 32);
-        if (!cuda(dmalloc((void**) &dWideScratch_, sizeof(float) * rowsCap * blockSize_), "cudaMalloc wide mix scratch")) return rc::CudaError;
-        if (!cuda(dmalloc((void**) &dWideTickets_, sizeof(unsigned int) * tick), "cudaMalloc wide mix tickets")) return rc::CudaError;
-        if (!cuda(dmemset(dWideTickets_, 0, sizeof(unsigned int) * tick), "memset wide mix tickets")) return rc::CudaError;
-        wideScratchRows_ = rowsCap;
-    }
+    if (!grow(dWideScratch_, wideScratchFloats_, (size_t) w.nScratch * blockSize_, "cudaMalloc wide mix scratch", false, 2) ||
+        !grow(dWideTickets_, wideTicketCount_, (size_t) w.nScratch * ((blockSize_ + 31) / 32), "cudaMalloc wide mix tickets", true, 2))
+        return rc::CudaError;
     return rc::Ok;
 }
 
 // The device half of a wide block after K1 / K3: per-voice outputs scattered to [voice][nOut] (every other channel zero), then K2w,
 // which also hands the mix bus to the host.
-int Engine::launchWide(size_t nOut, size_t numSamples, bool materialise, bool mix) {
+int Engine::launchWide(const BlockIO& io) {
     WidePlan& w = wide_;
-    if (materialise && dOutVoice_) {
+    const size_t nOut = io.nOut, numSamples = io.numSamples;
+    if (io.voiceOut) {
         // The channels no root of a voice aims at stay zero from block to block: the whole buffer is cleared only when the rows the
         // scatter writes (or nOut) changed, or something else wrote it since (the narrow path, a reallocation).
         if (!w.outZeroValid || w.outZeroNOut != nOut || w.outZeroRows != w.dstRow) {
@@ -2828,13 +2743,12 @@ int Engine::launchWide(size_t nOut, size_t numSamples, bool materialise, bool mi
         if (!cuda(launch_voice_out_scatter(dOutCompact_, w.dDst, (int) w.dstRow.size(), dOutVoice_, blockSize_, (int) numSamples, stream_), "voice out scatter launch")) return rc::CudaError;
         if (!w.dstRow.empty() && numSamples) ++launches_;
     }
-    if (mix) {
+    if (io.mix) {
         auto ev = timedBegin();
         const int nBig = (int) w.segs.size() - w.nSmall;
-        float* const mixDst = offlineMix_ ? offlineMix_ + offlineOffset_ : dMix_;
-        if (!cuda(launch_mix_reduce_wide(dPartial_, w.dRows, w.dSegs, w.nSmall, nBig, (int) nOut, mixDst, offlineMix_ ? offlineStride_ : blockSize_,
+        if (!cuda(launch_mix_reduce_wide(dPartial_, w.dRows, w.dSegs, w.nSmall, nBig, (int) nOut, io.mix + io.col, io.mixPitch,
                                          dWideScratch_, dWideTickets_, blockSize_, (int) numSamples, stream_, takeDeliver()), "wide mix reduce launch")) return rc::CudaError;
-        if (timeKernels_) { cudaEventRecord(ev.second, stream_); timedMixEvents_.push_back(ev); }
+        timedEnd(ev, 1);
         launches_ += (w.nSmall > 0) + (nBig > 0);
     }
     return rc::Ok;
@@ -2858,6 +2772,12 @@ std::pair<cudaEvent_t, cudaEvent_t> Engine::timedBegin() {
     return ev;
 }
 
+void Engine::timedEnd(std::pair<cudaEvent_t, cudaEvent_t> ev, int kind) {
+    if (!timeKernels_) return;
+    cudaEventRecord(ev.second, stream_);
+    timed_[kind].push_back(ev);
+}
+
 int Engine::peerBarrier() {
     Lock lk(mu_);
     if (planOnly_ || !peerAttached_ || peer_.world <= 1) return rc::Ok;
@@ -2870,17 +2790,15 @@ double Engine::takeKernelTimeMs(uint64_t* count) {
     Lock lk(mu_);
     if (planOnly_) { if (count) *count = 0; return 0.0; }
     cudaStreamSynchronize(stream_);
-    std::vector<std::pair<cudaEvent_t, cudaEvent_t>>* lists[4] = {&timedEvents_, &timedMixEvents_, &timedConvEvents_, &timedXchgEvents_};
     for (int k = 0; k < 4; ++k) {
-        lastKindMs_[k] = 0.0; lastKindCount_[k] = lists[k]->size();
-        for (auto& ev : *lists[k]) {
+        lastKindMs_[k] = 0.0; lastKindCount_[k] = timed_[k].size();
+        for (auto& ev : timed_[k]) {
             float ms = 0.0f;
             if (cudaEventElapsedTime(&ms, ev.first, ev.second) == cudaSuccess) lastKindMs_[k] += ms;
             eventPool_.push_back(ev);
         }
-        lists[k]->clear();
+        timed_[k].clear();
     }
-    lastConvMs_ = lastKindMs_[2]; lastConvCount_ = lastKindCount_[2];
     if (count) *count = lastKindCount_[0];
     return lastKindMs_[0];
 }
@@ -2905,23 +2823,6 @@ int Engine::processOffline(const float* const* in, size_t nIn, const float* inVo
     return offlineLoop(nIn ? in : nullptr, nIn, nIn ? inVoices : nullptr, mixOut, voicesOut, nOut, numSamples, chunkBlocks, sampleTime);
 }
 
-int Engine::ensureOfflineBuf(OfflineBuf& b, size_t floats) {
-    if (floats <= b.floats) return rc::Ok;
-    dsync();
-    for (int i = 0; i < 2; ++i) {
-        if (b.dev[i]) cudaFree(b.dev[i]);
-        if (b.pinned[i]) cudaFreeHost(b.pinned[i]);
-        b.dev[i] = nullptr; b.pinned[i] = nullptr;
-    }
-    b.floats = 0;
-    for (int i = 0; i < 2; ++i) {
-        if (!cuda(cudaMalloc((void**) &b.dev[i], floats * sizeof(float)), "cudaMalloc offline chunk")) return rc::CudaError;
-        if (!cuda(cudaMallocHost((void**) &b.pinned[i], floats * sizeof(float)), "cudaMallocHost offline chunk")) return rc::CudaError;
-    }
-    b.floats = floats;
-    return rc::Ok;
-}
-
 // The chunk loop of both offline entry points (the engine lock is held).  Blocks are enqueued back to back with no host synchronisation in
 // between; chunk buffers of C blocks per row carry the inputs up and the outputs down, two of each on the device and two PINNED on the host.
 // The user's buffers are pageable and strided; a 2-D copy straight from or into them would be staged by the driver row by row,
@@ -2941,10 +2842,13 @@ int Engine::offlineLoop(const float* const* in, size_t nIn, const float* inVoice
     while (C > 1 && maxRows * C * bs * sizeof(float) > ((size_t) 256 << 20)) C >>= 1;       // two chunk buffers of at most 256 MiB each
     if (C > numBlocks) C = numBlocks;
     const size_t W = C * bs, numChunks = (numBlocks + C - 1) / C;                           // W: floats per chunk row
-    int r = rc::Ok;
-    if (outRows && (r = ensureOfflineBuf(offOut_, outRows * W)) != rc::Ok) return r;
-    if (inRows && (r = ensureOfflineBuf(offIn_, inRows * W)) != rc::Ok) return r;
-    if (mixRows && (r = ensureOfflineBuf(offMix_, mixRows * W)) != rc::Ok) return r;
+    auto ensure = [&](OfflineBuf& b, size_t floats) {
+        for (int i = 0; i < 2; ++i)
+            if (!grow(b.dev[i], b.devFloats[i], floats, "cudaMalloc offline chunk") ||
+                !grow(b.pinned[i], b.pinnedFloats[i], floats, "cudaMallocHost offline chunk", false, 1, true)) return false;
+        return true;
+    };
+    if ((outRows && !ensure(offOut_, outRows * W)) || (inRows && !ensure(offIn_, inRows * W)) || (mixRows && !ensure(offMix_, mixRows * W))) return rc::CudaError;
     cudaStream_t copyStream = nullptr, upStream = nullptr;
     cudaEvent_t rendered[2] = {nullptr, nullptr}, copied[2] = {nullptr, nullptr}, uploaded[2] = {nullptr, nullptr};
     int rcode = rc::Ok;
@@ -2981,6 +2885,9 @@ int Engine::offlineLoop(const float* const* in, size_t nIn, const float* inVoice
             std::memcpy(mixOut[c] + s0, offMix_.pinned[pc.slot] + c * W, width * sizeof(float));
     };
     if (inRows && !stage(0)) rcode = rc::CudaError;
+    BlockIO io;                                                                                 // block b: column b % C of its chunk's slot
+    io.nIn = nIn; io.nOut = nOut; io.numSamples = bs; io.perVoiceIn = perVoiceIn;
+    io.inPitch = io.outPitch = io.mixPitch = (int) W;
     for (size_t b = 0; b < numBlocks && rcode == rc::Ok; ++b) {
         const size_t chunk = b / C, inChunk = b % C;
         const int slot = (int) (chunk & 1);
@@ -2989,11 +2896,11 @@ int Engine::offlineLoop(const float* const* in, size_t nIn, const float* inVoice
             if (inRows) cudaStreamWaitEvent(stream_, uploaded[slot], 0);                         // this chunk's inputs have arrived
         }
         if (sampleTime) sampleTime_ = *sampleTime + (int64_t) (b * bs);                          // as process() with userData, block by block
-        offlineOut_ = outRows ? offOut_.dev[slot] : nullptr;
-        offlineIn_ = inRows ? offIn_.dev[slot] : nullptr;
-        offlineMix_ = mixRows ? offMix_.dev[slot] : nullptr;
-        offlineStride_ = (int) W; offlineOffset_ = (int) (inChunk * bs);
-        rcode = enqueueBlock(nIn, nOut, bs, perVoiceIn, outRows != 0, mixRows != 0);
+        io.in = inRows ? offIn_.dev[slot] : nullptr;
+        io.voiceOut = outRows ? offOut_.dev[slot] : nullptr;
+        io.mix = mixRows ? offMix_.dev[slot] : nullptr;
+        io.col = (int) (inChunk * bs);
+        rcode = enqueueBlock(io);
         const bool lastOfChunk = inChunk + 1 == C || b + 1 == numBlocks;
         if (rcode == rc::Ok && lastOfChunk) {
             // the pinned buffers of this slot were scattered when chunk - 1 was enqueued (below), i.e. before these copies are issued
@@ -3009,7 +2916,7 @@ int Engine::offlineLoop(const float* const* in, size_t nIn, const float* inVoice
         }
     }
     if (rcode == rc::Ok) scatter(prev);
-    offlineOut_ = nullptr; offlineIn_ = nullptr; offlineMix_ = nullptr; offlineStride_ = 0; offlineOffset_ = 0; steadyValid_ = false;
+    steadyValid_ = false;
     cudaStreamSynchronize(stream_);
     if (copyStream) { cudaStreamSynchronize(copyStream); cudaStreamDestroy(copyStream); }
     if (upStream) { cudaStreamSynchronize(upStream); cudaStreamDestroy(upStream); }
@@ -3040,12 +2947,7 @@ int Engine::process(const float* const* in, size_t nIn, float* const* out, size_
         dsetdev();
         if (sampleTime) sampleTime_ = *sampleTime;   // BlockContext::userData as the wasm host passes it (wasm/Main.cpp:206-215)
         if (numSamples > (size_t) blockSize_) return fail(rc::BadArgument, "numSamples > blockSize");
-        const size_t need = (nIn + nOut) * blockSize_;
-        if (need > pinnedFloats_) {
-            if (hPinned_) { dsync(); cudaFreeHost(hPinned_); }
-            if (!cuda(cudaMallocHost(&hPinned_, sizeof(float) * need), "cudaMallocHost")) return rc::CudaError;
-            pinnedFloats_ = need;
-        }
+        if (!grow(hPinned_, pinnedFloats_, (nIn + nOut) * blockSize_, "cudaMallocHost", false, 1, true)) return rc::CudaError;
         if (nIn) {
             float* d = sharedInDevicePtr(nIn);
             if (!d) return rc::CudaError;

@@ -264,7 +264,7 @@ public:
     // CUDA events recorded on the launching stream (option "time_kernels" = 1). Synchronises the stream.
     double takeKernelTimeMs(uint64_t* count);
     // K3 time/count gathered by the same takeKernelTimeMs() call
-    double lastConvolveTimeMs(uint64_t* count) const { Lock lk(mu_); if (count) *count = lastConvCount_; return lastConvMs_; }
+    double lastConvolveTimeMs(uint64_t* count) const { Lock lk(mu_); if (count) *count = lastKindCount_[2]; return lastKindMs_[2]; }
     // per kernel kind (0 = K1 render, 1 = K2 mix reduce, 2 = K3 convolve, 3 = K4 mix exchange): summed ms and launch counts of the same call
     void lastKernelTimes(double ms[4], uint64_t counts[4]) const { Lock lk(mu_); for (int i = 0; i < 4; ++i) { ms[i] = lastKindMs_[i]; counts[i] = lastKindCount_[i]; } }
     // A cross-GPU barrier on the render stream (K4 with an empty payload): returns once every rank's stream has reached it.
@@ -307,10 +307,10 @@ private:
     uint64_t launches_ = 0;
     int64_t sampleTime_ = 0;
     bool timeKernels_ = false;
-    std::vector<std::pair<cudaEvent_t, cudaEvent_t>> timedEvents_, timedConvEvents_, timedMixEvents_, timedXchgEvents_, eventPool_;
-    double lastConvMs_ = 0.0; uint64_t lastConvCount_ = 0;
+    std::vector<std::pair<cudaEvent_t, cudaEvent_t>> timed_[4], eventPool_;   // timed_[kind]: K1, K2, K3, K4 pairs since takeKernelTimeMs()
     double lastKindMs_[4] = {0, 0, 0, 0}; uint64_t lastKindCount_[4] = {0, 0, 0, 0};   // K1, K2, K3, K4 of the latest takeKernelTimeMs()
     std::pair<cudaEvent_t, cudaEvent_t> timedBegin();
+    void timedEnd(std::pair<cudaEvent_t, cudaEvent_t> ev, int kind);
 
     // I/O staging
     float* dMix_ = nullptr;          // [max(MAX_OUT, widest nOut so far)][blockSize]
@@ -330,14 +330,31 @@ private:
     bool hostDeliver_ = true, processAllReduce_ = true;   // options "host_deliver", "process_allreduce"
     bool deliverArmed_ = false, deliverLaunched_ = false;
     HostDeliver takeDeliver();
+    void allocMixHost();
     // Offline chunk buffers, kept across calls: two on the device (rendered into / uploaded to back to back), two pinned on the host
-    struct OfflineBuf { float* dev[2] = {nullptr, nullptr}; float* pinned[2] = {nullptr, nullptr}; size_t floats = 0; };
+    struct OfflineBuf { float* dev[2] = {nullptr, nullptr}; float* pinned[2] = {nullptr, nullptr}; size_t devFloats[2] = {0, 0}, pinnedFloats[2] = {0, 0}; };
     OfflineBuf offOut_, offIn_, offMix_;  // per-voice outputs [voice][nOut][C * bs], inputs [nIn][C * bs] or [voice][nIn][C * bs], mix [nOut][C * bs]
-    int ensureOfflineBuf(OfflineBuf& b, size_t floats);
     int offlineLoop(const float* const* in, size_t nIn, const float* inVoices, float* const* mixOut, float* voicesOut,
                     size_t nOut, size_t numSamples, size_t chunkBlocks, const int64_t* sampleTime);
-    size_t curNOut_ = 0;
-    struct BatchBuffers { LaunchParams* dDescs = nullptr; int* dTileStart = nullptr; size_t capGroups = 0; std::vector<char> lastDescs; };
+    // Where a block's I/O lives: rows of `pitch` floats, the block in column `col` of each.  Device-resident calls pass the engine's own
+    // buffers (pitch blockSize, column 0), offline blocks their chunk slots.
+    struct BlockIO {
+        size_t nIn = 0, nOut = 0, numSamples = 0;
+        bool perVoiceIn = false, allReduce = false;
+        const float* in = nullptr; int inPitch = 0;    // [nIn] or [voice][nIn] rows (null without inputs)
+        float* voiceOut = nullptr; int outPitch = 0;   // [voice][nOut] rows; null: per-voice outputs are not materialised
+        float* mix = nullptr; int mixPitch = 0;        // [nOut] rows; null: no mix
+        int col = 0;
+        // The steady-state key: the cached descriptors hold the input and output base pointers and pitches; the column and the mix rows
+        // are kernel arguments of every block (K1's many-groups launches, K2, K2w), so they may differ.
+        bool sameSteadyKey(const BlockIO& o) const {
+            return nIn == o.nIn && nOut == o.nOut && numSamples == o.numSamples && perVoiceIn == o.perVoiceIn && allReduce == o.allReduce &&
+                   in == o.in && inPitch == o.inPitch && voiceOut == o.voiceOut && outPitch == o.outPitch && !mix == !o.mix;
+        }
+    };
+    int enqueueBlock(const BlockIO& io);
+    int walkGroups(const BlockIO& io);
+    struct BatchBuffers { LaunchParams* dDescs = nullptr; int* dTileStart = nullptr; size_t capDescs = 0, capTiles = 0; std::vector<char> lastDescs; };
     std::map<int, BatchBuffers> batch_;   // per tile width
     // Steady-state fast path for engines made of many batched voice groups (BASELINE config 5: 1250 graphs): when the last block found
     // every group steady — no queued program, nothing dirty, all root fades settled, no event mirrors to advance — and the call has the
@@ -347,8 +364,8 @@ private:
     static constexpr int PIPE_BUCKET = 1000;   // bucket key = tile width (+ PIPE_BUCKET for pipelined one-voice programs)
     std::vector<SteadyBucket> steadyBuckets_;
     bool steadyValid_ = false;
-    size_t steadyKey_[7] = {0, 0, 0, 0, 0, 0, 0};
-    int steadyTiles_ = 0;
+    BlockIO steadyIO_;
+    int steadyTiles_ = 0;                 // tiles of the last walk: K2's partial rows
     // Wide mix bus (nOut > MAX_OUT_CHANNELS, DESIGN.md section 3): each voice group writes compact partial rows for the channels its
     // roots aim at only (mix channels, ascending), per-voice outputs go to a compact [voice][mix channel] buffer and are scattered to
     // [voice][nOut]; K2w reduces each channel over its own row list.  Rebuilt by every slow pass; the device copies are re-uploaded
@@ -366,16 +383,13 @@ private:
         // the per-voice output buffer is zero outside outZeroRows (rows of [voice][outZeroNOut]) since its last clear
         bool outZeroValid = false; size_t outZeroNOut = 0; std::vector<int> outZeroRows;
     } wide_;
-    float* dWideScratch_ = nullptr; unsigned int* dWideTickets_ = nullptr; size_t wideScratchRows_ = 0;
+    float* dWideScratch_ = nullptr; unsigned int* dWideTickets_ = nullptr; size_t wideScratchFloats_ = 0, wideTicketCount_ = 0;
     float* dOutCompact_ = nullptr; size_t outCompactFloats_ = 0;
     size_t mixFloats_ = 0;                // dMix_ and the mapped host-delivery buffer hold this many floats
     int uploadWidePlan();
-    int launchWide(size_t nOut, size_t numSamples, bool materialise, bool mix);
+    int launchWide(const BlockIO& io);
     // the mix channels of a program: distinct channels in [0, nOut) of all its roots, running or fading, ascending
     std::vector<int> mixChannels(const Group& g, const Program& p, size_t nOut) const;
-    // Offline blocks: where materialised outputs, inputs and the mix bus are instead of dOutVoice_, dInShared_ / dInVoice_ and dMix_ (chunk
-    // buffers of rows of offlineStride_ floats; this block's column starts at offlineOffset_)
-    float* offlineOut_ = nullptr; const float* offlineIn_ = nullptr; float* offlineMix_ = nullptr; int offlineStride_ = 0, offlineOffset_ = 0;
 
     // K4 state
     void* dExchange_ = nullptr; size_t exchangeBytes_ = 0; size_t exchangeFlagOffset_ = 0, exchangeOwnOffset_ = 0;
@@ -389,6 +403,10 @@ private:
     cudaError_t dmemset(void* p, int v, size_t bytes);
     cudaError_t dmemcpy(void* dst, const void* src, size_t bytes, cudaMemcpyKind kind);
     cudaError_t dmemcpySync(void* dst, const void* src, size_t bytes, cudaMemcpyKind kind);
+    cudaError_t dzeroBlock(float* p, int pitch, size_t rows);   // the first blockSize floats of `rows` rows of `pitch` floats
+    // Grow a device allocation (pinned: page-locked host memory) holding cap elements to at least n, allocating n * slack: drains the
+    // stream, drops the old contents, zeroes the new memory on request.  false (p null, cap 0) when the allocation fails.
+    template <typename T> bool grow(T*& p, size_t& cap, size_t n, const char* what, bool zero = false, size_t slack = 1, bool pinned = false);
     void dsync();
     void dsetdev();
     int fail(int code, const std::string& msg) { lastError_ = msg; return code; }
@@ -418,7 +436,6 @@ private:
     int compile(Group& g, int nIn, std::shared_ptr<Program>& out);
     void traverse(Group& g, std::set<int32_t>& visited, std::vector<int32_t>& order, int32_t n);
     int chooseTileWidth(int nv) const;
-    int ensureBuffers(size_t nIn, size_t nOut, bool perVoiceIn, bool materialise, size_t wideRows = 0, size_t wideOutRows = 0);
     friend struct Compiler;
 };
 
