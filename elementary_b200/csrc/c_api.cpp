@@ -102,6 +102,14 @@ int elem_b200_process_offline(elem_b200_runtime* rt, const float* const* in, siz
     GUARD(rt->engine->processOffline(in, nIn, inVoices, mixOut, voicesOut, nOut, numSamples, chunkBlocks, static_cast<const int64_t*>(userData)));
 }
 
+int elem_b200_process_offline_events(elem_b200_runtime* rt, const float* const* in, size_t nIn, const float* inVoices,
+                                     float* const* mixOut, float* voicesOut, size_t nOut, size_t numSamples,
+                                     size_t chunkBlocks, void* userData, int voiceBegin, int voiceEnd,
+                                     elem_b200_block_event_cb cb, void* user) {
+    GUARD(rt->engine->processOfflineEvents(in, nIn, inVoices, mixOut, voicesOut, nOut, numSamples, chunkBlocks, static_cast<const int64_t*>(userData),
+                                           voiceBegin, voiceEnd, cb, user));
+}
+
 int elem_b200_enqueue_block(elem_b200_runtime* rt, size_t nIn, size_t nOut, size_t numSamples, int flags) {
     GUARD(rt->engine->enqueueBlock(nIn, nOut, numSamples, (flags & 1) != 0, (flags & 2) != 0, (flags & 4) != 0, (flags & 8) != 0));
 }

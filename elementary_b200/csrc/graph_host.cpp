@@ -230,7 +230,7 @@ Engine::~Engine() {
     if (dInShared_) dfree(dInShared_);
     if (hPinned_ && !planOnly_) cudaFreeHost(hPinned_);
     if (hMixHost_) cudaFreeHost(hMixHost_);
-    for (OfflineBuf* b : {&offOut_, &offIn_, &offMix_})
+    for (OfflineBuf* b : {&offOut_, &offIn_, &offMix_, &offLog_})
         for (int i = 0; i < 2; ++i) { if (b->dev[i]) cudaFree(b->dev[i]); if (b->pinned[i]) cudaFreeHost(b->pinned[i]); }
     if (dDeliverDone_) cudaFree(dDeliverDone_);
     if (wide_.dRows) dfree(wide_.dRows);
@@ -2810,9 +2810,8 @@ int Engine::renderOffline(size_t nOut, size_t numBlocks, float* hostOut, size_t 
     return offlineLoop(nullptr, 0, nullptr, nullptr, hostOut, nOut, numBlocks * (size_t) blockSize_, chunkBlocks, nullptr);
 }
 
-int Engine::processOffline(const float* const* in, size_t nIn, const float* inVoices, float* const* mixOut, float* voicesOut,
-                           size_t nOut, size_t numSamples, size_t chunkBlocks, const int64_t* sampleTime) {
-    Lock lk(mu_);
+// The arguments every offline call with inputs checks, before rendering anything (the engine lock is held).
+int Engine::offlineArgs(const float* const* in, size_t nIn, const float* inVoices, float* voicesOut, size_t nOut) {
     if (in && inVoices) return fail(rc::BadArgument, "processOffline: shared and per-voice inputs are exclusive");
     if (nIn > 0 && !in && !inVoices) return fail(rc::BadArgument, "processOffline: nIn > 0 without inputs");
     if (nOut == 0 || nOut > (size_t) MAX_WIDE_OUT_CHANNELS || (voicesOut && nOut > (size_t) MAX_OUT_CHANNELS))
@@ -2820,7 +2819,29 @@ int Engine::processOffline(const float* const* in, size_t nIn, const float* inVo
     if (processAllReduce_ && peerAttached_ && peer_.world > 1)
         return fail(rc::BadArgument, "processOffline: the mix bus is not summed across GPUs offline (option process_allreduce = 0 renders this rank alone)");
     if (planOnly_) return fail(rc::CudaError, "plan-only runtime (no CUDA device): rendering is impossible, there is no CPU fallback");
+    return rc::Ok;
+}
+
+int Engine::processOffline(const float* const* in, size_t nIn, const float* inVoices, float* const* mixOut, float* voicesOut,
+                           size_t nOut, size_t numSamples, size_t chunkBlocks, const int64_t* sampleTime) {
+    Lock lk(mu_);
+    const int r = offlineArgs(in, nIn, inVoices, voicesOut, nOut);
+    if (r != rc::Ok) return r;
     return offlineLoop(nIn ? in : nullptr, nIn, nIn ? inVoices : nullptr, mixOut, voicesOut, nOut, numSamples, chunkBlocks, sampleTime);
+}
+
+int Engine::processOfflineEvents(const float* const* in, size_t nIn, const float* inVoices, float* const* mixOut, float* voicesOut,
+                                 size_t nOut, size_t numSamples, size_t chunkBlocks, const int64_t* sampleTime, int vb, int ve,
+                                 BlockEventFn cb, void* user) {
+    Lock lk(mu_);
+    if (!cb) return fail(rc::BadArgument, "processOfflineEvents: no event callback");
+    if (vb < 0 || vb > numVoices_ || ve > numVoices_ || (ve >= 0 && ve < vb))
+        return fail(rc::BadArgument, "processOfflineEvents: the voice range is out of bounds");
+    const int r = offlineArgs(in, nIn, inVoices, voicesOut, nOut);
+    if (r != rc::Ok) return r;
+    EventLog log;
+    log.vb = vb; log.ve = ve; log.cb = cb; log.user = user;
+    return offlineLoop(nIn ? in : nullptr, nIn, nIn ? inVoices : nullptr, mixOut, voicesOut, nOut, numSamples, chunkBlocks, sampleTime, &log);
 }
 
 // The chunk loop of both offline entry points (the engine lock is held).  Blocks are enqueued back to back with no host synchronisation in
@@ -2828,9 +2849,10 @@ int Engine::processOffline(const float* const* in, size_t nIn, const float* inVo
 // The user's buffers are pageable and strided; a 2-D copy straight from or into them would be staged by the driver row by row,
 // synchronously.  So a chunk travels as ONE contiguous async copy between pinned and device memory, and this thread moves rows between the
 // user's buffers and pinned memory while the GPU renders: it fills chunk k + 1's inputs (uploaded on their own stream) and scatters
-// chunk k - 1's outputs while chunk k renders.
+// chunk k - 1's outputs while chunk k renders.  With an event log, K5 follows every block, the log travels down with the chunk's outputs
+// and its events are delivered once the chunk is scattered.
 int Engine::offlineLoop(const float* const* in, size_t nIn, const float* inVoices, float* const* mixOut, float* voicesOut,
-                        size_t nOut, size_t numSamples, size_t chunkBlocks, const int64_t* sampleTime) {
+                        size_t nOut, size_t numSamples, size_t chunkBlocks, const int64_t* sampleTime, EventLog* log) {
     dsetdev();
     const size_t bs = (size_t) blockSize_, numBlocks = (numSamples + bs - 1) / bs;
     if (numBlocks == 0) return rc::Ok;
@@ -2838,8 +2860,13 @@ int Engine::offlineLoop(const float* const* in, size_t nIn, const float* inVoice
     const size_t inRows = perVoiceIn ? (size_t) numVoices_ * nIn : (in ? nIn : 0);
     const size_t outRows = voicesOut ? (size_t) numVoices_ * nOut : 0, mixRows = mixOut ? nOut : 0;
     const size_t maxRows = std::max(inRows, std::max(outRows, mixRows));
+    if (log) {
+        const int r = eventLogBegin(*log);
+        if (r != rc::Ok) return r;
+    }
+    const size_t blockFloats = std::max(maxRows * bs, log ? log->blockWords : 0);           // the largest chunk buffer, per block
     size_t C = chunkBlocks ? chunkBlocks : 8;
-    while (C > 1 && maxRows * C * bs * sizeof(float) > ((size_t) 256 << 20)) C >>= 1;       // two chunk buffers of at most 256 MiB each
+    while (C > 1 && blockFloats * C * sizeof(float) > ((size_t) 256 << 20)) C >>= 1;        // two chunk buffers of at most 256 MiB each
     if (C > numBlocks) C = numBlocks;
     const size_t W = C * bs, numChunks = (numBlocks + C - 1) / C;                           // W: floats per chunk row
     auto ensure = [&](OfflineBuf& b, size_t floats) {
@@ -2848,7 +2875,8 @@ int Engine::offlineLoop(const float* const* in, size_t nIn, const float* inVoice
                 !grow(b.pinned[i], b.pinnedFloats[i], floats, "cudaMallocHost offline chunk", false, 1, true)) return false;
         return true;
     };
-    if ((outRows && !ensure(offOut_, outRows * W)) || (inRows && !ensure(offIn_, inRows * W)) || (mixRows && !ensure(offMix_, mixRows * W))) return rc::CudaError;
+    if ((outRows && !ensure(offOut_, outRows * W)) || (inRows && !ensure(offIn_, inRows * W)) || (mixRows && !ensure(offMix_, mixRows * W)) ||
+        (log && log->blockWords && !ensure(offLog_, log->blockWords * C))) return rc::CudaError;
     cudaStream_t copyStream = nullptr, upStream = nullptr;
     cudaEvent_t rendered[2] = {nullptr, nullptr}, copied[2] = {nullptr, nullptr}, uploaded[2] = {nullptr, nullptr};
     int rcode = rc::Ok;
@@ -2883,6 +2911,7 @@ int Engine::offlineLoop(const float* const* in, size_t nIn, const float* inVoice
             std::memcpy(voicesOut + row * numSamples + s0, offOut_.pinned[pc.slot] + row * W, width * sizeof(float));
         for (size_t c = 0; c < mixRows; ++c)
             std::memcpy(mixOut[c] + s0, offMix_.pinned[pc.slot] + c * W, width * sizeof(float));
+        if (log) rcode = eventLogReplay(*log, pc.slot, pc.chunk * C);
     };
     if (inRows && !stage(0)) rcode = rc::CudaError;
     BlockIO io;                                                                                 // block b: column b % C of its chunk's slot
@@ -2901,6 +2930,7 @@ int Engine::offlineLoop(const float* const* in, size_t nIn, const float* inVoice
         io.mix = mixRows ? offMix_.dev[slot] : nullptr;
         io.col = (int) (inChunk * bs);
         rcode = enqueueBlock(io);
+        if (rcode == rc::Ok && log) rcode = eventLogBlock(*log, slot, inChunk);
         const bool lastOfChunk = inChunk + 1 == C || b + 1 == numBlocks;
         if (rcode == rc::Ok && lastOfChunk) {
             // the pinned buffers of this slot were scattered when chunk - 1 was enqueued (below), i.e. before these copies are issued
@@ -2908,6 +2938,7 @@ int Engine::offlineLoop(const float* const* in, size_t nIn, const float* inVoice
             cudaStreamWaitEvent(copyStream, rendered[slot], 0);
             if (outRows && !cuda(cudaMemcpyAsync(offOut_.pinned[slot], offOut_.dev[slot], outRows * W * sizeof(float), cudaMemcpyDeviceToHost, copyStream), "D2H offline chunk")) rcode = rc::CudaError;
             if (mixRows && !cuda(cudaMemcpyAsync(offMix_.pinned[slot], offMix_.dev[slot], mixRows * W * sizeof(float), cudaMemcpyDeviceToHost, copyStream), "D2H offline mix chunk")) rcode = rc::CudaError;
+            if (log && log->used[slot] && !cuda(cudaMemcpyAsync(offLog_.pinned[slot], offLog_.dev[slot], log->used[slot] * sizeof(uint32_t), cudaMemcpyDeviceToHost, copyStream), "D2H offline event log")) rcode = rc::CudaError;
             cudaEventRecord(copied[slot], copyStream);
             if (rcode == rc::Ok && inRows && chunk + 1 < numChunks && !stage(chunk + 1)) rcode = rc::CudaError;   // overlaps with this chunk's render
             Pending cur; cur.valid = true; cur.chunk = chunk; cur.blocks = inChunk + 1; cur.slot = slot;

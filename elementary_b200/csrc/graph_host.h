@@ -229,6 +229,14 @@ public:
     // block; sampleTime: as process()'s, for the first block (block k gets *sampleTime + k * blockSize).
     int processOffline(const float* const* in, size_t nIn, const float* inVoices, float* const* mixOut, float* voicesOut,
                        size_t nOut, size_t numSamples, size_t chunkBlocks, const int64_t* sampleTime);
+    // processOffline that also delivers, for block k of the call, cb(k, type, event JSON, user) for every event that
+    // processQueuedEvents(vb, ve) would deliver right after the k-th of the equivalent process() calls (ve < 0: all voices).  A K5 launch
+    // after each block logs what that poll reads and applies its side effects on the device; the log travels with the chunk's outputs and
+    // is replayed through the live poll's formatter after the chunk is scattered, so callbacks lag the render by up to two chunks.
+    typedef void (*BlockEventFn)(size_t block, const char* type, const char* json, void* user);
+    int processOfflineEvents(const float* const* in, size_t nIn, const float* inVoices, float* const* mixOut, float* voicesOut,
+                             size_t nOut, size_t numSamples, size_t chunkBlocks, const int64_t* sampleTime, int vb, int ve,
+                             BlockEventFn cb, void* user);
 
     // Cross-GPU mix bus (SURVEY.md §8e): peerExport() allocates this rank's exchange buffer and returns its CUDA IPC handle
     // (64 bytes); peerAttach() maps the buffers of all ranks (handles = world x 64 bytes, in rank order).  Afterwards
@@ -334,8 +342,41 @@ private:
     // Offline chunk buffers, kept across calls: two on the device (rendered into / uploaded to back to back), two pinned on the host
     struct OfflineBuf { float* dev[2] = {nullptr, nullptr}; float* pinned[2] = {nullptr, nullptr}; size_t devFloats[2] = {0, 0}, pinnedFloats[2] = {0, 0}; };
     OfflineBuf offOut_, offIn_, offMix_;  // per-voice outputs [voice][nOut][C * bs], inputs [nIn][C * bs] or [voice][nIn][C * bs], mix [nOut][C * bs]
+    OfflineBuf offLog_;                   // event log of the chunk's blocks, packed (EventLog)
+
+    // A poll (processQueuedEvents) in two halves.  planPoll walks the polled event nodes and takes the decisions that are the same for every
+    // voice of a group — whether a scope / fft window is read and where, the metro flag — advancing the host mirrors; emitPoll reads what
+    // the item needs from a PollSource (the device now, or a block's logged record) and turns it into events, with the capture relays.
+    struct PollItem {
+        Group* g = nullptr; Node* n = nullptr;
+        int b = 0, e = 0;                 // group-relative voices
+        bool fire = false;                // scope / fft: a window is read; metro: the flag was up
+        uint32_t r = 0, size = 0;         // scope / fft: read position, window length
+        int nch = 0;                      // scope / fft: ring channels read
+        size_t logOff = 0;                // offline: the item's record in the chunk's event log (words)
+    };
+    struct PollSource;
+    struct DeviceSource;
+    struct LogSource;
+    template <class F> int forEachPolled(int vb, int ve, bool queued, F&& f);
+    int planPoll(int vb, int ve, std::vector<PollItem>& items);
+    int emitPoll(const PollItem& it, PollSource& src, EventFn cb, void* user);
+    size_t pollRecordWords(const PollItem& it) const;   // the item's record in the event log
+    int captureConsumed(const PollItem& it, bool clearReady);
+    // The per-block event log of an offline render: the plans of the blocks of the two chunks in flight and their records' extent.
+    struct EventLog {
+        int vb = 0, ve = 0;
+        BlockEventFn cb = nullptr; void* user = nullptr;
+        size_t blockWords = 0;            // bound on one block's records
+        std::vector<std::vector<PollItem>> blocks[2];
+        size_t used[2] = {0, 0};
+    };
+    int offlineArgs(const float* const* in, size_t nIn, const float* inVoices, float* voicesOut, size_t nOut);
+    int eventLogBegin(EventLog& log);
+    int eventLogBlock(EventLog& log, int slot, size_t inChunk);
+    int eventLogReplay(EventLog& log, int slot, size_t firstBlock);
     int offlineLoop(const float* const* in, size_t nIn, const float* inVoices, float* const* mixOut, float* voicesOut,
-                    size_t nOut, size_t numSamples, size_t chunkBlocks, const int64_t* sampleTime);
+                    size_t nOut, size_t numSamples, size_t chunkBlocks, const int64_t* sampleTime, EventLog* log = nullptr);
     // Where a block's I/O lives: rows of `pitch` floats, the block in column `col` of each.  Device-resident calls pass the engine's own
     // buffers (pitch blockSize, column 0), offline blocks their chunk slots.
     struct BlockIO {

@@ -75,6 +75,27 @@ struct PeerMix {
 };
 cudaError_t launch_mix_exchange(const PeerMix& pm, float* mix, int count, uint32_t epoch, int* status, cudaStream_t stream, HostDeliver hd = HostDeliver{});
 
+// K5 (event_log_kernel.cu): the per-block event log of an offline render with events.  After a block renders, one launch copies what a
+// poll after that block would read into the chunk's event log and applies the poll's side effects, so that the device state evolves as
+// under a process() + processQueuedEvents() loop.  One item per polled event node, voices [b, b + n) of its group:
+//   EVLOG_ROWS     meter / snapshot: log [3][n] words of state rows 0..2 (the readouts, the push count); zero the push count
+//   EVLOG_CAPTURE  capture: log [3][n] words of state rows 2..4 (write position, read position, relay-ready flag), then [n][lim] floats:
+//                  the ring's samples [r, w) of each voice (at most lim); set the read position to w and clear the flag
+//   EVLOG_WINDOW   scope / fft: log [tile t0..t1)[channel < nch][size][L] floats, the ring window at read position r (no side effect)
+enum EventLogKind : int { EVLOG_ROWS = 0, EVLOG_CAPTURE = 1, EVLOG_WINDOW = 2 };
+struct EventLogItem {
+    uint32_t* rows;           // the node's first state row (row j of voice v: rows[j * Vpad + v])
+    const float* ring;        // capture: [tile][ringFloats][L]; scope / fft: [tile][ringCh][SCOPE_RING][L]
+    uint32_t* log;            // where this item's record starts
+    int kind, b, n, Vpad, L;
+    uint32_t cap, lim, ringFloats;   // capture: ring capacity (a power of two), samples logged per voice at most, ring + scratch floats per lane
+    uint32_t r, size;         // window: read position, window length
+    int ringCh, nch, t0, t1;  // window: channels of the ring, channels logged, tiles
+};
+constexpr int EVENT_LOG_BATCH = 32;   // items per launch (the batch travels as one kernel parameter)
+struct EventLogBatch { int n; EventLogItem item[EVENT_LOG_BATCH]; };
+cudaError_t launch_event_log(const EventLogBatch& batch, cudaStream_t stream);
+
 // A/B builds (-DEB_OPPROF): cycles / dispatches per opcode of the interpreter; zeros in the product library.
 cudaError_t debug_opprof_read(unsigned long long* out128, bool reset);
 

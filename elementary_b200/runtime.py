@@ -38,6 +38,7 @@ _lib = None
 
 
 EVENT_CB = C.CFUNCTYPE(None, C.c_char_p, C.c_char_p, C.c_void_p)
+BLOCK_EVENT_CB = C.CFUNCTYPE(None, C.c_size_t, C.c_char_p, C.c_char_p, C.c_void_p)
 
 
 def load_library() -> C.CDLL:
@@ -74,6 +75,9 @@ def load_library() -> C.CDLL:
     lib.elem_b200_process_offline.restype = C.c_int
     lib.elem_b200_process_offline.argtypes = [C.c_void_p, _f32pp, C.c_size_t, _f32p, _f32pp, _f32p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p]
     lib.elem_b200_enqueue_block.restype = C.c_int
+    lib.elem_b200_process_offline_events.restype = C.c_int
+    lib.elem_b200_process_offline_events.argtypes = [C.c_void_p, _f32pp, C.c_size_t, _f32p, _f32pp, _f32p, C.c_size_t, C.c_size_t, C.c_size_t,
+                                                     C.c_void_p, C.c_int, C.c_int, BLOCK_EVENT_CB, C.c_void_p]
     lib.elem_b200_enqueue_block.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int]
     lib.elem_b200_peer_export.restype = C.c_int
     lib.elem_b200_peer_export.argtypes = [C.c_void_p, C.c_char_p]
@@ -275,11 +279,16 @@ class Runtime:
 
     def process_offline(self, inputs: Optional[np.ndarray] = None, num_outputs: int = 1, num_samples: Optional[int] = None,
                         voice_inputs: Optional[np.ndarray] = None, want_mix: bool = True, want_voices: bool = False,
-                        chunk_blocks: int = 0, sample_time: Optional[int] = None):
+                        chunk_blocks: int = 0, sample_time: Optional[int] = None, on_event=None,
+                        event_voices: Optional[Sequence[int]] = None):
         """OfflineRenderer.process (js/packages/offline-renderer/index.ts:87-133): ceil(n / block_size) full blocks in one call, with
         ``inputs`` [n_in, n] broadcast to every voice or ``voice_inputs`` [voice, n_in, n] (zero past n), no host round trip per block.
         ``num_samples`` defaults to the inputs' length (one block without inputs).  ``sample_time``: as for :meth:`process`, for the
-        first block.  Returns (mix [n_out, n] | None, voices [voice, n_out, n] | None), truncated to n."""
+        first block.  Returns (mix [n_out, n] | None, voices [voice, n_out, n] | None), truncated to n.
+
+        ``on_event(block, type, event_dict)``: every block's events, as :meth:`process_queued_events` (``voices`` = ``event_voices``)
+        would report them right after the block (elem_b200_process_offline_events); called in block order before the call returns,
+        and it must not call into this runtime.  An exception it raises is re-raised once the call has returned."""
         if inputs is not None and voice_inputs is not None:
             raise ValueError("process_offline: give inputs or voice_inputs, not both")
         src = inputs if inputs is not None else voice_inputs
@@ -299,9 +308,28 @@ class Runtime:
         ov = np.zeros((self.num_voices, num_outputs, n), dtype=np.float32) if want_voices else None
         mix_ptrs = (_f32p * max(1, num_outputs))(*[mix[i].ctypes.data_as(_f32p) for i in range(num_outputs)]) if want_mix else None
         user = None if sample_time is None else C.byref(C.c_int64(int(sample_time)))
-        rc = self._lib.elem_b200_process_offline(self._h, in_ptrs, n_in, vin_ptr, mix_ptrs,
-                                                 ov.ctypes.data_as(_f32p) if ov is not None else None,
-                                                 num_outputs, n, int(chunk_blocks), user)
+        ov_ptr = ov.ctypes.data_as(_f32p) if ov is not None else None
+        if on_event is None:
+            rc = self._lib.elem_b200_process_offline(self._h, in_ptrs, n_in, vin_ptr, mix_ptrs, ov_ptr, num_outputs, n, int(chunk_blocks), user)
+            self._check(rc, "process_offline")
+            return mix, ov
+        import json as _json
+        raised: List[BaseException] = []
+
+        def _cb(block, type_, js, _user):
+            if raised:
+                return
+            try:
+                on_event(int(block), type_.decode(), _json.loads(js.decode()))
+            except BaseException as exc:    # ctypes cannot unwind through C: keep the first one for after the call
+                raised.append(exc)
+
+        cb = BLOCK_EVENT_CB(_cb)
+        vb, ve = (0, -1) if event_voices is None else (int(event_voices[0]), int(event_voices[1]))
+        rc = self._lib.elem_b200_process_offline_events(self._h, in_ptrs, n_in, vin_ptr, mix_ptrs, ov_ptr, num_outputs, n,
+                                                        int(chunk_blocks), user, vb, ve, cb, None)
+        if raised:
+            raise raised[0]
         self._check(rc, "process_offline")
         return mix, ov
 

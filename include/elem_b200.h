@@ -126,7 +126,8 @@ int elem_b200_render_offline(elem_b200_runtime* rt, size_t nOut, size_t numBlock
  *   running root aims at is +0.0); per-voice outputs nOut <= 8.  With voicesOut == NULL nothing per-voice is materialised or copied.
  * SAMPLE CLOCK: userData NULL lets the engine clock run on; a pointer to an int64 t0 gives block k the time t0 + k * blockSize, as if
  *   elem_b200_process had been called with that userData for each block.
- * EVENTS are not polled inside the call: afterwards the event queues hold what as many elem_b200_process calls would have left.
+ * EVENTS are not polled inside the call: afterwards the event queues hold what as many elem_b200_process calls would have left
+ *   (elem_b200_process_offline_events delivers them block by block).
  * Blocks go through chunk buffers of chunkBlocks blocks (0 = default 8; fewer when a chunk buffer would pass 256 MiB): chunk k + 1's
  *   inputs are uploaded and chunk k - 1's outputs copied out while chunk k renders.  The engine lock is held for the whole call.
  * Returns -2, before rendering anything, when both `in` and `inVoices` are given, when nIn > 0 comes without an input pointer, when
@@ -134,6 +135,29 @@ int elem_b200_render_offline(elem_b200_runtime* rt, size_t nOut, size_t numBlock
  *   offline mix is not summed across GPUs. */
 int elem_b200_process_offline(elem_b200_runtime* rt, const float* const* in, size_t nIn, const float* inVoices,
                               float* const* mixOut, float* voicesOut, size_t nOut, size_t numSamples, size_t chunkBlocks, void* userData);
+
+/* elem_b200_process_offline with every block's events, as OfflineRenderer.process does when it polls after each block
+ * (js/packages/offline-renderer/index.ts:104-132).  Arguments, blocks, chunks, sample clock, outputs and errors are those of
+ * elem_b200_process_offline, and the outputs are bit for bit what it returns: logging events does not change the audio.
+ * EVENTS: for block k of this call (0-based), cb(k, type, jsonEvent, user) receives the events, in the same order and with the same text,
+ *   that elem_b200_process_queued_events_range(rt, voiceBegin, voiceEnd, ...) would deliver right after the k-th of the equivalent
+ *   elem_b200_process calls (voiceEnd < 0: all voices; voiceBegin == voiceEnd: none).  After each block a kernel copies what that poll reads
+ *   (meter / snapshot readouts, the capture samples written since the last poll, scope / fft windows when one is due) into an event log that
+ *   travels down with the chunk's outputs, and applies the poll's effects on the device (queues drained, capture read positions moved).
+ *   The chunk size shrinks so that two logs stay within 256 MiB each, like the other chunk buffers.
+ * DELIVERY: in block order, on the calling thread, before the call returns; up to two chunks after the block rendered.  The engine lock is
+ *   held throughout, so cb must not call into the runtime.
+ * STATE AFTERWARDS: queues, scope / fft read positions, capture relays and the metro flag are what the process() + poll-per-block loop
+ *   leaves; voices outside [voiceBegin, voiceEnd) keep what un-polled process() calls leave them, with the group-wide scope / fft / metro
+ *   rule of elem_b200_process_queued_events_range.  Capture samples that wait in the ring when the call starts are read into the relay
+ *   first (reported with the next relay), so a backlog within one block of the ring's 2^k capacity keeps samples the live poll would lose.
+ * Returns -2, before rendering anything, where elem_b200_process_offline does, for cb == NULL, and for a voice range outside
+ *   [0, numVoices] or with voiceEnd < voiceBegin. */
+typedef void (*elem_b200_block_event_cb)(size_t block, const char* type, const char* jsonEvent, void* user);
+int elem_b200_process_offline_events(elem_b200_runtime* rt, const float* const* in, size_t nIn, const float* inVoices,
+                                     float* const* mixOut, float* voicesOut, size_t nOut, size_t numSamples,
+                                     size_t chunkBlocks, void* userData, int voiceBegin, int voiceEnd,
+                                     elem_b200_block_event_cb cb, void* user);
 
 /* Device-resident stepping for throughput measurement and pipelines that keep audio in HBM: enqueue one block
  * on the engine's stream (no host copies, no synchronisation).  flags: 1 = read per-voice inputs from
