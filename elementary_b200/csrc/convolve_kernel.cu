@@ -5,7 +5,7 @@
 // Persistent CTAs (2 per SM; a TMA producer warp, 4 MAC warps, 4 transform warps) walk the channel pairs; a pair shares one
 // pass over the IR spectra so that every IR spectrum value fetched from L2 is reused.  Per pair and call:
 //   1. append the new samples to the partition's input buffer, zero-pad to 1024 (FFTConvolver.cpp:157-164)
-//   2. real FFT 1024 = complex Stockham radix-2 FFT 512 in shared memory + split post-pass  (replaces OouraFFT::fft,
+//   2. real FFT 1024 = complex Stockham radix-4 FFT 512 in shared memory + split post-pass  (replaces OouraFFT::fft,
 //      AudioFFT.cpp:132-155; float arithmetic instead of the reference's double)
 //   3. if the input buffer was empty: Ypre = sum_{i>=1} H_i * X_{cur+i}   (FFTConvolver.cpp:168-177,
 //      ComplexMultiplyAccumulate Utilities.cpp:66-117)
@@ -73,14 +73,8 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 // T transforms pair n+1 and pair n-1: the HBM stream of a CTA only ever waits for data, not for transforms.
 constexpr int TM_GROUP = 128;                       // threads per worker group
 constexpr int TM_THREADS = 2 * TM_GROUP + 32;       // T + M + producer warp
-#ifndef EB_CONV_TM_STAGES
-#define EB_CONV_TM_STAGES 5   /* 5 x 12 KB + 44 KB = 104 KB per CTA, two CTAs per SM still fit in 228 KB */
-#endif
-#ifndef EB_CONV_TM_CTAS
-#define EB_CONV_TM_CTAS 2
-#endif
-constexpr int TM_STAGES = EB_CONV_TM_STAGES;
-constexpr int TM_CTAS_PER_SM = EB_CONV_TM_CTAS;
+constexpr int TM_STAGES = 5;                        // 5 x 12 KB + 44 KB = 104 KB per CTA, two CTAs per SM still fit in 228 KB
+constexpr int TM_CTAS_PER_SM = 2;
 // The per-channel-IR form streams CH input rows and up to CH IR rows per stage (16 KB): 4 stages x 16 KB + 44 KB = 108 KB per CTA,
 // two CTAs per SM still fit in 228 KB (5 stages would not).
 constexpr int PC_STAGES = 4;
@@ -99,14 +93,10 @@ __device__ __forceinline__ void tgroup_sync() { asm volatile("bar.sync 2, %0;" :
 // Complex FFT 512 (Stockham autosort, out of place between two shared-memory buffers), 128 threads: four radix-4 stages — one
 // butterfly per thread and channel, sub-transform length p = 1, 4, 16, 64 — and a final radix-2 stage (p = 256, two butterflies per
 // thread): 5 group barriers instead of the 9 of a pure radix-2 transform.  tw[m] = exp(-2 pi i m / 1024), m < 512.  Result in `b`.
-#ifndef EB_CONV_RADIX4
-#define EB_CONV_RADIX4 1      /* 0 = the radix-2 transform (9 group barriers instead of 5) */
-#endif
 template <bool INVERSE>
 __device__ __forceinline__ void fft512_t(float2 (*a)[N2], float2 (*b)[N2], const float2* tw, int t) {
     float2 (*src)[N2] = a;
     float2 (*dst)[N2] = b;
-#if EB_CONV_RADIX4
 #pragma unroll 1
     for (int p = 1; p < N2 / 2; p <<= 2) {
         const int k = t & (p - 1);
@@ -152,28 +142,6 @@ __device__ __forceinline__ void fft512_t(float2 (*a)[N2], float2 (*b)[N2], const
         }
         tgroup_sync();
     }
-#else
-#pragma unroll 1
-    for (int ns = 1; ns < N2; ns <<= 1) {
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int bi = t + h * TM_GROUP;                 // butterfly index 0..255
-            const int k = bi & (ns - 1);
-            float2 w = tw[k * (N2 / ns)];
-            if (INVERSE) w.y = -w.y;
-            const int j0 = ((bi - k) << 1) + k;
-#pragma unroll
-            for (int c = 0; c < CH; ++c) {
-                const float2 u = src[c][bi];
-                const float2 v = cmul(w, src[c][bi + N2 / 2]);
-                dst[c][j0] = cadd(u, v);
-                dst[c][j0 + ns] = csub(u, v);
-            }
-        }
-        tgroup_sync();
-        float2 (*tmp)[N2] = src; src = dst; dst = tmp;
-    }
-#endif
 }
 
 // Relayout of a grown input spectra ring (convolve.h convolver_relayout): one CTA of 128 threads per (channel, new slot).
@@ -230,11 +198,8 @@ __global__ void __launch_bounds__(TM_THREADS, TM_CTAS_PER_SM) convolve_chunk_tm_
         }
     };
     auto unitS = [&](int u) { return PER_CH ? units[u].z : S; };
-#ifndef EB_CONV_EARLY_PRODUCER
-#define EB_CONV_EARLY_PRODUCER 1   /* 0 = the producer starts behind the CTA barrier like everyone else */
-#endif
     // The producer thread initialises the barriers itself and fills the first ring stages BEFORE the CTA-wide barrier: the delay line
-    // is on its way from HBM while the other warps still fetch the twiddle table (cold after an L2 flush).  Its first TM_STAGES
+    // is on its way from HBM while the other warps still fetch the twiddle table (cold after an L2 flush).  Its first STAGES
     // stages need no `empty` wait (fresh barriers pass the parity-1 wait), so nothing it touches depends on the other warps yet.
     const bool producerThread = (tid == 2 * TM_GROUP);
     uint32_t pit = 0;                    // producer: stages issued so far
@@ -274,12 +239,12 @@ __global__ void __launch_bounds__(TM_THREADS, TM_CTAS_PER_SM) convolve_chunk_tm_
         if (++pi >= puS) { pi = 1; pu += gridDim.x; skipEmpty(); }
     };
     const bool streams = fill == 0 && (PER_CH || S > 1);
-    if (EB_CONV_EARLY_PRODUCER ? producerThread : (tid == 0)) {
+    if (producerThread) {
         for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], TM_GROUP / 32); }
         for (int i = 0; i < 2; ++i) { mbar_init(&xfull[i], 1); mbar_init(&xempty[i], TM_GROUP / 32); mbar_init(&yfull[i], TM_GROUP / 32); mbar_init(&yempty[i], 1); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
         fence_proxy_async();
-        if (EB_CONV_EARLY_PRODUCER && streams) {
+        if (streams) {
             skipEmpty();
             for (int k = 0; k < STAGES && pu < numUnits; ++k) produceOne();
         }
@@ -290,7 +255,6 @@ __global__ void __launch_bounds__(TM_THREADS, TM_CTAS_PER_SM) convolve_chunk_tm_
     if (tid >= 2 * TM_GROUP) {
         // ---------------- producer warp ----------------
         if (producerThread && streams) {
-            if (!EB_CONV_EARLY_PRODUCER) skipEmpty();
             while (pu < numUnits) produceOne();
         }
         return;
@@ -593,13 +557,10 @@ cudaError_t convolver_process_chunk(ConvolverState& st, const float* in, int inS
         if (smCount <= 0) smCount = 132;
     }
     const int persistent = smCount * TM_CTAS_PER_SM;                   // a multiple of the SM count: one resident wave
-#ifndef EB_CONV_BALANCED
-#define EB_CONV_BALANCED 1      /* 0 = always the full resident wave */
-#endif
     // Every CTA walks the same number of channel pairs: 512 pairs on 264 resident CTAs (H100: 132 SMs x 2) would leave 16 CTAs idle for
     // the second half of the kernel (248 CTAs hold two pairs, 16 hold one); 256 CTAs with two pairs each keep the HBM stream full until the end.
     int grid = units < persistent ? units : persistent;
-    if (EB_CONV_BALANCED && units > persistent) {
+    if (units > persistent) {
         const int rounds = (units + persistent - 1) / persistent;
         grid = (units + rounds - 1) / rounds;
     }

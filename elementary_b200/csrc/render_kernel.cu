@@ -39,9 +39,7 @@ namespace eb {
 namespace {
 
 constexpr float kEps = FLT_EPSILON;
-#ifndef EB_SVF_SCAN_MAX_L
-#define EB_SVF_SCAN_MAX_L 4      // tiles of up to this many voices run the svf tick as a register-blocked warp scan (render_ops.inc, OP_SVF)
-#endif
+constexpr int kSvfScanMaxL = 4;   // tiles of up to this many voices run the svf tick as a register-blocked warp scan (render_ops.inc, OP_SVF)
 constexpr unsigned FULL = 0xFFFFFFFFu;
 
 // Everything the interpreter touches per sample lives in the CTA's dynamic shared memory.  Addresses into it are kept as 32-bit
@@ -90,15 +88,6 @@ struct Opnd {
 
 #define LDE(o, k) ((o).p[(k) * (o).stride])
 #define LDT(o, t) ((o).p[(t) * (o).tstride])
-// the same read by ANY lane of the voice column (an operand pointer is set up for the owner lane = lane vlane of the column;
-// parameter operands, stride 0, already point at the column)
-#define LDC(o, t) ((o).p[(t) * (o).tstride + ((o).stride ? (vlane - lane) : 0)])
-#ifndef EB_RECUR_BROADCAST
-#define EB_RECUR_BROADCAST 0      /* narrow-tile recurrences: 0 = operands by shuffle from the lane that holds them, 1 = broadcast reads of the slots */
-#endif
-#ifndef EB_INTERP_PREFETCH
-#define EB_INTERP_PREFETCH 0      /* interpreter loop: 1 = next op's header + operand words loaded while the current op runs */
-#endif
 
 __device__ __forceinline__ float clampf(float v, float lo, float hi) { return (v < lo) ? lo : ((hi < v) ? hi : v); }
 __device__ __forceinline__ double clampd(double v, double lo, double hi) { return (v < lo) ? lo : ((hi < v) ? hi : v); }
@@ -524,8 +513,17 @@ __device__ __noinline__ void ctl_capture(const CtlCtx& c) {
 
 // A/B builds only (-DEB_OPPROF, tools/opprof.py): cycles and dispatch count per opcode, accumulated by lane 0 of every warp of
 // the interpreter — what the host's pipeline cost model (graph_host.cpp) is calibrated against.  Not compiled into the product library.
+// OPPROF_OP_BEGIN / OPPROF_OP_END bracket one op dispatch of either op loop of render_tile.
 #ifdef EB_OPPROF
 __device__ unsigned long long g_opprof[2 * 64];
+#define OPPROF_OP_BEGIN() const long long prof_t0 = clock64()
+#define OPPROF_OP_END(opcode) do { \
+        __syncwarp(); \
+        if (lane == 0) { atomicAdd(&g_opprof[2 * ((opcode) & 63)], (unsigned long long) (clock64() - prof_t0)); atomicAdd(&g_opprof[2 * ((opcode) & 63) + 1], 1ull); } \
+    } while (0)
+#else
+#define OPPROF_OP_BEGIN() ((void) 0)
+#define OPPROF_OP_END(opcode) ((void) 0)
 #endif
 
 // =========================================================================================================
@@ -641,10 +639,9 @@ __device__ __forceinline__ void render_tile(const LaunchParams& P, const int til
 #define T_OF(k) (tlane + (k) * PER)                       /* sample index of this lane's element in slice k */
 #define FOR_OWNER(t) _Pragma("unroll 4") for (int t = 0; t < cnt; ++t)
     // recurrences walked by every lane of a voice column (narrow tiles, render_ops.inc OP_POLE): sample t = k * PER + j of the column
-    // lives in register k of lane j * L + vlane
+    // lives in register k of lane j * L + vlane, and FETCH_T(register k, j) hands it to every lane of the column
     // (the j loop stays ROLLED: the interpreter is instruction-fetch bound, 32 unrolled steps of shuffles run 3x slower than a rolled
     // loop that stays in the instruction cache)
-#define FOR_TJ(k, j) _Pragma("unroll") for (int k = 0; k < NITER; ++k) _Pragma("unroll 4") for (int j = 0, jn_ = min(PER, cnt - k * PER); j < jn_; ++j)
 #define FETCH_T(reg, j) __shfl_sync(FULL, (reg), (j) * L + vlane)
 
 #ifdef EB_OPPROF
@@ -703,14 +700,9 @@ __device__ __forceinline__ void render_tile(const LaunchParams& P, const int til
 #define CHAIN_NEXT(s) ((void) 0)
 #define PC_ADVANCE(n) ((void) 0)
 #define PC_SKIP_SEGMENT_IF(cond, n) ((void) 0)
-#ifdef EB_OPPROF
-                            const long long prof_t0 = clock64();
-#endif
+                            OPPROF_OP_BEGIN();
 #include "render_ops.inc"
-#ifdef EB_OPPROF
-                            __syncwarp();
-                            if (lane == 0) { atomicAdd(&g_opprof[2 * (opcode & 63)], (unsigned long long) (clock64() - prof_t0)); atomicAdd(&g_opprof[2 * (opcode & 63) + 1], 1ull); }
-#endif
+                            OPPROF_OP_END(opcode);
 #undef CHAIN_NEXT
 #undef OPWORD
 #undef CHAIN_FOR_STEPS
@@ -725,63 +717,6 @@ __device__ __forceinline__ void render_tile(const LaunchParams& P, const int til
                 }
             };
             run.template operator()<0, EB_SPEC_CODE_LEN>(run);
-        }
-#else
-#if EB_INTERP_PREFETCH
-        // The interpreter loop is software-pipelined: the header (two 128-bit words) and the first four operand words of the NEXT op are
-        // loaded while the current op executes, so that a dispatch does not begin with three dependent trips to memory (header ->
-        // operand word -> slot).  Ops that move the program counter themselves (phasor runs, skipped segments) just reload.
-        const uint32_t* pc = P.code + ((PIPE && pipeW > 1) ? P.pipeCode[stage] : 0u);
-        uint4 h0 = __ldg(reinterpret_cast<const uint4*>(pc));
-        uint4 h1 = __ldg(reinterpret_cast<const uint4*>(pc + 4));
-        uint4 ow4 = __ldg(reinterpret_cast<const uint4*>(pc + 8));      // (behind the last op lie the END header's zero words: always readable)
-        for (;;) {
-            __syncwarp();   // slot / state traffic of the previous op is visible to every lane
-            const uint32_t opcode = h0.x & 0xFF;
-            if (opcode == OP_END) break;
-            const uint32_t nwords = (h0.x >> 8) & 0xFF, mode = h0.x >> 24;
-            const SP out = slots + (SLOTI((int) ((h0.x >> 16) & 0xFF)) * E + lane);    // element k of this lane: out[k * 32]
-            const SP outT = out;                                         // owner lane, sample t: outT[t * L]
-            const uint32_t sidx = h0.y, aux0 = h0.z, aux1 = h0.w;
-            const uint64_t ptrbits = (uint64_t) h1.x | ((uint64_t) h1.y << 32);
-            const uint32_t count6 = h1.z;
-            const uint32_t* opnds = pc + OP_HEADER_WORDS;
-            const uint4 ow = ow4;
-            pc += OP_HEADER_WORDS + nwords;
-            const uint32_t* const pcPrefetched = pc;
-            const uint4 h0n = __ldg(reinterpret_cast<const uint4*>(pc));
-            const uint4 h1n = __ldg(reinterpret_cast<const uint4*>(pc + 4));
-            const uint4 ow4n = __ldg(reinterpret_cast<const uint4*>(pc + 8));
-
-            // program-word access of the interpreter (render_ops.inc explains the contract)
-#define OPWORD(i) (((i) == 0) ? ow.x : ((i) == 1) ? ow.y : ((i) == 2) ? ow.z : ((i) == 3) ? ow.w : __ldg(opnds + (i)))
-#define CHAIN_FOR_STEPS(s) const uint32_t* sp = opnds + 1; uint32_t cfw_ = ow.y, cow_ = ow.z; for (uint32_t s = 0; s < count6; ++s, sp += 2)
-#define CHAIN_FN_WORD(s) cfw_
-#define CHAIN_OPND_WORD(s) cow_
-#define CHAIN_NEXT(s) do { cfw_ = __ldg(sp + 2); cow_ = __ldg(sp + 3); } while (0)
-#define PC_ADVANCE(n) pc += (n)
-#define PC_SKIP_SEGMENT_IF(cond, n) if (cond) pc += (n)
-#ifdef EB_OPPROF
-            const long long prof_t0 = clock64();
-#endif
-#include "render_ops.inc"
-#ifdef EB_OPPROF
-            __syncwarp();
-            if (lane == 0) { atomicAdd(&g_opprof[2 * (opcode & 63)], (unsigned long long) (clock64() - prof_t0)); atomicAdd(&g_opprof[2 * (opcode & 63) + 1], 1ull); }
-#endif
-#undef OPWORD
-#undef CHAIN_FOR_STEPS
-#undef CHAIN_FN_WORD
-#undef CHAIN_OPND_WORD
-#undef CHAIN_NEXT
-#undef PC_ADVANCE
-#undef PC_SKIP_SEGMENT_IF
-            if (pc == pcPrefetched) { h0 = h0n; h1 = h1n; ow4 = ow4n; }
-            else {
-                h0 = __ldg(reinterpret_cast<const uint4*>(pc));
-                h1 = __ldg(reinterpret_cast<const uint4*>(pc + 4));
-                ow4 = __ldg(reinterpret_cast<const uint4*>(pc + 8));
-            }
         }
 #else
         const uint32_t* pc = P.code + ((PIPE && pipeW > 1) ? P.pipeCode[stage] : 0u);
@@ -808,14 +743,9 @@ __device__ __forceinline__ void render_tile(const LaunchParams& P, const int til
 #define CHAIN_NEXT(s) do { cfw_ = __ldg(sp + 2); cow_ = __ldg(sp + 3); } while (0)
 #define PC_ADVANCE(n) pc += (n)
 #define PC_SKIP_SEGMENT_IF(cond, n) if (cond) pc += (n)
-#ifdef EB_OPPROF
-            const long long prof_t0 = clock64();
-#endif
+            OPPROF_OP_BEGIN();
 #include "render_ops.inc"
-#ifdef EB_OPPROF
-            __syncwarp();
-            if (lane == 0) { atomicAdd(&g_opprof[2 * (opcode & 63)], (unsigned long long) (clock64() - prof_t0)); atomicAdd(&g_opprof[2 * (opcode & 63) + 1], 1ull); }
-#endif
+            OPPROF_OP_END(opcode);
 #undef OPWORD
 #undef CHAIN_FOR_STEPS
 #undef CHAIN_FN_WORD
@@ -824,7 +754,6 @@ __device__ __forceinline__ void render_tile(const LaunchParams& P, const int til
 #undef PC_ADVANCE
 #undef PC_SKIP_SEGMENT_IF
         }
-#endif   // EB_INTERP_PREFETCH
 #endif   // EB_SPEC_PROGRAM
 
         if constexpr (PIPE) {
@@ -866,8 +795,6 @@ __device__ __forceinline__ void render_tile(const LaunchParams& P, const int til
 
 #ifdef EB_OPPROF
     if (lane == 0) { atomicAdd(&g_opprof[2 * 63], (unsigned long long) (clock64() - prof_tile0)); atomicAdd(&g_opprof[2 * 63 + 1], 1ull); }   // whole sample loop of one warp
-#endif
-#ifdef EB_OPPROF
     const long long prof_wb0 = clock64();
 #endif
     // ---- state rows shared memory -> HBM, in the form of the staging prologue ----
@@ -936,23 +863,17 @@ __device__ __forceinline__ void render_tile(const LaunchParams& P, const int til
 #undef FOR_K
 #undef T_OF
 #undef FOR_OWNER
-#undef FOR_TJ
 #undef FETCH_T
 }
 
 // Occupancy target: the full-width geometry (L = 32, every lane a voice)
 // is issue-latency bound and gains 20 % from 64-register / 8-CTA occupancy; the narrow geometries run few warps
 // anyway and prefer the 128-register budget.
-#ifndef EB_L32_MINBLOCKS
-#define EB_L32_MINBLOCKS 8
-#endif
-#ifndef EB_L1_MINBLOCKS
-#define EB_L1_MINBLOCKS 4
-#endif
+constexpr int kL32MinBlocks = 8, kL1MinBlocks = 4;
 #ifndef EB_NARROW_MINBLOCKS
 #define EB_NARROW_MINBLOCKS 4      /* 1 < L < 32; a specialised kernel may be compiled for 8 (64 registers): engine option "spec_minblocks" */
 #endif
-#define EB_BOUNDS __launch_bounds__(128, (LOGL == 5) ? EB_L32_MINBLOCKS : ((LOGL == 0) ? EB_L1_MINBLOCKS : EB_NARROW_MINBLOCKS))
+#define EB_BOUNDS __launch_bounds__(128, (LOGL == 5) ? kL32MinBlocks : ((LOGL == 0) ? kL1MinBlocks : EB_NARROW_MINBLOCKS))
 
 // One voice group per launch: the descriptor travels in the constant bank.
 template <int NITER, int LOGL>
@@ -964,6 +885,16 @@ __global__ void EB_BOUNDS render_block_kernel(const __grid_constant__ LaunchPara
     render_tile<NITER, LOGL>(P, tile, perWarp, P.sampleTime, 0, 0);   // (offline chunks: the host pre-offsets the I/O pointers)
 }
 
+// The voice group of tile w in a many-groups launch: the largest g with tileStart[g] <= w (binary search in the tile prefix table).
+__device__ __forceinline__ int group_of_tile(const int* tileStart, int nGroups, int w) {
+    int lo = 0, hi = nGroups - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (__ldg(tileStart + mid) <= w) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
 // Many voice groups (different graphs) of the same tile geometry in ONE launch: warp w finds its group by binary
 // search in the tile prefix table and reads that group's descriptor from global memory.  This is what makes
 // thousands of small heterogeneous graphs (BASELINE config 5) run concurrently instead of one launch each.
@@ -973,13 +904,9 @@ __global__ void EB_BOUNDS render_groups_kernel(const LaunchParams* __restrict__ 
                                                 const int inOffset) {
     const int w = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (w >= totalTiles) return;
-    int lo = 0, hi = nGroups - 1;                      // largest g with tileStart[g] <= w
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (__ldg(tileStart + mid) <= w) lo = mid; else hi = mid - 1;
-    }
+    const int g = group_of_tile(tileStart, nGroups, w);
     // the sample clock and the I/O columns of an offline chunk travel as arguments: the descriptors of a steady engine never change
-    render_tile<NITER, LOGL>(descs[lo], w - __ldg(tileStart + lo), perWarp, sampleTime, outOffset, inOffset);
+    render_tile<NITER, LOGL>(descs[g], w - __ldg(tileStart + g), perWarp, sampleTime, outOffset, inOffset);
 }
 
 // The same for one-voice graphs whose programs the host cut into pipeline stages (LaunchParams::pipeW): ONE CTA per graph, warp w of
@@ -995,14 +922,10 @@ __global__ void __launch_bounds__(32 * MAX_PIPE, 8) render_groups_pipe_kernel(co
     if (threadIdx.x < MAX_PIPE) reinterpret_cast<volatile int*>(g_smem + perGraph)[threadIdx.x] = 0;   // progress counters
     __syncthreads();
     if (w >= totalTiles) return;
-    int lo = 0, hi = nGroups - 1;                      // largest g with tileStart[g] <= w
-    while (lo < hi) {
-        const int mid = (lo + hi + 1) >> 1;
-        if (__ldg(tileStart + mid) <= w) lo = mid; else hi = mid - 1;
-    }
-    const LaunchParams& P = descs[lo];
+    const int g = group_of_tile(tileStart, nGroups, w);
+    const LaunchParams& P = descs[g];
     if (stage >= max(1, P.pipeW)) return;              // (whole warps leave; no CTA-wide barrier follows)
-    render_tile<NITER, 0, true>(P, w - __ldg(tileStart + lo), perGraph, sampleTime, outOffset, inOffset, stage);
+    render_tile<NITER, 0, true>(P, w - __ldg(tileStart + g), perGraph, sampleTime, outOffset, inOffset, stage);
 }
 
 #ifndef __CUDACC_RTC__   // K2, K4 and the host launchers are not needed by a run-time compiled specialisation of K1
@@ -1107,26 +1030,20 @@ size_t render_smem_bytes(int nSlots, int nOut, int nStateRows, int nParams, int 
     return (size_t) warpsPerCta * perWarp * sizeof(float);
 }
 
-template <int NITER, int LOGL>
-static cudaError_t launch_impl(const LaunchParams& P, int grid, int threads, size_t smem, cudaStream_t stream) {
-    cudaError_t e = cudaFuncSetAttribute(render_block_kernel<NITER, LOGL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
-    if (e != cudaSuccess) return e;
-    // per-warp area = everything in front of the (optional) staged table
-    const size_t warpArea = P.tableSmem >= 0 ? (size_t) P.tableSmem * sizeof(float) : smem;
-    render_block_kernel<NITER, LOGL><<<grid, threads, smem, stream>>>(P, (int) (warpArea / sizeof(float) / (threads / 32)));
-    return cudaGetLastError();
-}
+// A K1 tile geometry as compile-time constants: E = 32 * NITER elements per sample tile, L = 1 << LOGL voices per warp.
+template <int NITER_, int LOGL_> struct RenderGeometry { static constexpr int NITER = NITER_, LOGL = LOGL_; };
 
-static cudaError_t launch_render_block_geometry(const LaunchParams& P, int L, int grid, int threads, size_t smem, int perWarpFloats, int niterOverride, cudaStream_t stream);
-
-template <int NITER, int LOGL>
-static cudaError_t launch_groups_impl(const LaunchParams* descs, const int* tileStart, int nGroups, int totalTiles,
-                                      int grid, int threads, size_t smem, long long sampleTime, int outOffset, int inOffset, cudaStream_t stream) {
-    cudaError_t e = cudaFuncSetAttribute(render_groups_kernel<NITER, LOGL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
-    if (e != cudaSuccess) return e;
-    render_groups_kernel<NITER, LOGL><<<grid, threads, smem, stream>>>(descs, tileStart, nGroups, totalTiles,
-                                                                          (int) (smem / sizeof(float) / (threads / 32)), sampleTime, outOffset, inOffset);
-    return cudaGetLastError();
+// Calls f(RenderGeometry<NITER, LOGL>{}) with NITER = render_niter_for(L, niterOverride) and LOGL = log2 L.  Every K1 launcher picks
+// its kernel here, so a voice group keeps its sample-tile length whichever launch runs it: a group that a live cut moves into the
+// batched launch must, or its samples change bits (the svf scan, for one, depends on the tile length).  The list is the
+// geometries the library is compiled for; any other is an error.
+template <typename F>
+static cudaError_t with_render_geometry(int L, int niterOverride, F&& f) {
+    const int niter = render_niter_for(L, niterOverride), logl = ilog2(L);
+#define GEOMETRY(N, LG) if (niter == N && logl == LG) return f(RenderGeometry<N, LG>{})
+    GEOMETRY(8, 5); GEOMETRY(4, 5); GEOMETRY(8, 4); GEOMETRY(8, 3); GEOMETRY(4, 2); GEOMETRY(8, 1); GEOMETRY(4, 1); GEOMETRY(4, 0); GEOMETRY(1, 0);
+#undef GEOMETRY
+    return cudaErrorInvalidValue;
 }
 
 cudaError_t launch_render_block(const LaunchParams& P, int warpsPerCta, int niterOverride, cudaStream_t stream, const SpecKernel* spec) {
@@ -1146,21 +1063,15 @@ cudaError_t launch_render_block(const LaunchParams& P, int warpsPerCta, int nite
         smem += (size_t) Q.tableFloats * 4 + 16;              // + the mbarrier
     } else { Q.tableSmem = -1; Q.tableSrc = nullptr; }
     if (spec && spec->function) return specialise_launch(*spec, Q, grid, threads, smem, perWarpFloats, stream);
-    return launch_render_block_geometry(Q, L, grid, threads, smem, perWarpFloats, niterOverride, stream);
-}
-
-static cudaError_t launch_render_block_geometry(const LaunchParams& P, int L, int grid, int threads, size_t smem, int perWarpFloats, int niterOverride, cudaStream_t stream) {
-    switch (L) {
-        case 32: return render_niter_for(32, niterOverride) == 4 ? launch_impl<4, 5>(P, grid, threads, smem, stream)
-                                                                  : launch_impl<8, 5>(P, grid, threads, smem, stream);
-        case 16: return launch_impl<8, 4>(P, grid, threads, smem, stream);
-        case 8:  return launch_impl<8, 3>(P, grid, threads, smem, stream);
-        case 4:  return launch_impl<4, 2>(P, grid, threads, smem, stream);
-        case 2:  return render_niter_for(2, niterOverride) == 8 ? launch_impl<8, 1>(P, grid, threads, smem, stream)
-                                                                 : launch_impl<4, 1>(P, grid, threads, smem, stream);
-        default: return render_niter_for(1, niterOverride) == 4 ? launch_impl<4, 0>(P, grid, threads, smem, stream)
-                                                                : launch_impl<1, 0>(P, grid, threads, smem, stream);
-    }
+    return with_render_geometry(L, niterOverride, [&](auto g) {
+        using G = decltype(g);
+        cudaError_t e = cudaFuncSetAttribute(render_block_kernel<G::NITER, G::LOGL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
+        if (e != cudaSuccess) return e;
+        // per-warp area = everything in front of the (optional) staged table
+        const size_t warpArea = Q.tableSmem >= 0 ? (size_t) Q.tableSmem * sizeof(float) : smem;
+        render_block_kernel<G::NITER, G::LOGL><<<grid, threads, smem, stream>>>(Q, (int) (warpArea / sizeof(float) / (threads / 32)));
+        return cudaGetLastError();
+    });
 }
 
 // descs / tileStart are DEVICE pointers; maxSlots etc. are the maxima over the groups (uniform shared-memory carve-up).
@@ -1170,23 +1081,15 @@ cudaError_t launch_render_groups(const LaunchParams* descs, const int* tileStart
     if (totalTiles <= 0) return cudaSuccess;
     const int grid = (totalTiles + warpsPerCta - 1) / warpsPerCta;
     const int threads = warpsPerCta * 32;
-    // the same sample-tile length as the single-group launch of the geometry (render_niter_for): a group that is cut keeps its
-    // tile length, so its samples stay the same bits (the svf scan, for one, depends on it)
     const size_t smem = render_smem_bytes(maxSlots, nOut, maxStateRows, maxParams, warpsPerCta, tileWidth, niterOverride);
-    if (tileWidth == 1 && render_niter_for(1, niterOverride) == 4)
-        return launch_groups_impl<4, 0>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, inOffset, stream);
-    if (tileWidth == 2 && render_niter_for(2, niterOverride) == 8)
-        return launch_groups_impl<8, 1>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, inOffset, stream);
-    if (tileWidth == 32 && render_niter_for(32, niterOverride) == 4)
-        return launch_groups_impl<4, 5>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, inOffset, stream);
-    switch (tileWidth) {
-        case 32: return launch_groups_impl<8, 5>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, inOffset, stream);
-        case 16: return launch_groups_impl<8, 4>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, inOffset, stream);
-        case 8:  return launch_groups_impl<8, 3>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, inOffset, stream);
-        case 4:  return launch_groups_impl<4, 2>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, inOffset, stream);
-        case 2:  return launch_groups_impl<4, 1>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, inOffset, stream);
-        default: return launch_groups_impl<1, 0>(descs, tileStart, nGroups, totalTiles, grid, threads, smem, sampleTime, outOffset, inOffset, stream);
-    }
+    return with_render_geometry(tileWidth, niterOverride, [&](auto g) {
+        using G = decltype(g);
+        cudaError_t e = cudaFuncSetAttribute(render_groups_kernel<G::NITER, G::LOGL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
+        if (e != cudaSuccess) return e;
+        render_groups_kernel<G::NITER, G::LOGL><<<grid, threads, smem, stream>>>(descs, tileStart, nGroups, totalTiles,
+                                                                                (int) (smem / sizeof(float) / (threads / 32)), sampleTime, outOffset, inOffset);
+        return cudaGetLastError();
+    });
 }
 
 // One CTA of `stages` warps per one-voice graph (descs / tileStart are DEVICE pointers; the maxima size the per-graph shared memory).
@@ -1198,13 +1101,17 @@ cudaError_t launch_render_groups_pipe(const LaunchParams* descs, const int* tile
     if (stages > MAX_PIPE) stages = MAX_PIPE;
     const size_t graphBytes = render_smem_bytes(maxSlots, nOut, maxStateRows, maxParams, 1, 1, niterOverride);
     const size_t smem = graphBytes + sizeof(int) * 8;              // + the progress counters
-    const bool wide = render_niter_for(1, niterOverride) == 4;
-    cudaError_t e = wide ? cudaFuncSetAttribute(render_groups_pipe_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem)
-                         : cudaFuncSetAttribute(render_groups_pipe_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
-    if (e != cudaSuccess) return e;
-    if (wide) render_groups_pipe_kernel<4><<<totalTiles, 32 * stages, smem, stream>>>(descs, tileStart, nGroups, totalTiles, (int) (graphBytes / sizeof(float)), sampleTime, outOffset, inOffset);
-    else render_groups_pipe_kernel<1><<<totalTiles, 32 * stages, smem, stream>>>(descs, tileStart, nGroups, totalTiles, (int) (graphBytes / sizeof(float)), sampleTime, outOffset, inOffset);
-    return cudaGetLastError();
+    return with_render_geometry(1, niterOverride, [&](auto g) -> cudaError_t {
+        using G = decltype(g);
+        if constexpr (G::LOGL != 0) return cudaErrorInvalidValue;   // (not reached: one-voice tiles)
+        else {
+            cudaError_t e = cudaFuncSetAttribute(render_groups_pipe_kernel<G::NITER>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
+            if (e != cudaSuccess) return e;
+            render_groups_pipe_kernel<G::NITER><<<totalTiles, 32 * stages, smem, stream>>>(descs, tileStart, nGroups, totalTiles, (int) (graphBytes / sizeof(float)),
+                                                                                         sampleTime, outOffset, inOffset);
+            return cudaGetLastError();
+        }
+    });
 }
 
 cudaError_t launch_mix_reduce(const float* partial, float* out, int outStride, float* scratch, unsigned int* tickets, int nTiles, int nOut,
