@@ -11,6 +11,7 @@
 #include <list>
 #include <sstream>
 #include <thread>
+#include <unordered_set>
 
 #include "convolve.h"
 #include "kernels.h"
@@ -1275,6 +1276,8 @@ void Engine::traverse(Group& g, std::set<int32_t>& visited, std::vector<int32_t>
     visited.insert(n);
 }
 
+constexpr uint32_t OP_HOST_CONV = 0xF0;   // host-only pseudo opcode of a Convolve node: lowered to STOREBUF + K3 + LOADBUF by the stage split
+
 struct Compiler {
     Engine& E;
     Group& g;
@@ -1289,17 +1292,75 @@ struct Compiler {
         struct Step { uint32_t fn; uint32_t kind; int32_t ref; };   // OP_CHAIN: acc = fn(acc, operand) / fn(acc)
         std::vector<Step> steps;
         std::vector<uint32_t> imm;         // raw immediate words behind the operands (control nodes)
-        int segment = 0;                   // root sub-sequence the op belongs to
+        int slot = 0;                      // output slot (allocateSlots)
         bool dead = false;                 // absorbed into a later chain
-        bool isSeg = false;
-        int segRoot = 0;
-        size_t segEndOp = 0;
     };
-    std::vector<PendingOp> ops;
+    using Segments = std::vector<std::vector<PendingOp>>;   // one op list per root, indexed by root index: the root's sub-sequence
+    Segments segs;
     std::vector<std::pair<int, int32_t>> promotes;   // (root index, tapOut node id)
     int32_t tempCounter = 0;
 
     int32_t newTemp() { return INT32_MIN + (++tempCounter); }
+
+    // device floats, zeroed; false with lastError set when CUDA fails
+    bool zeroedFloats(float*& p, size_t floats, const char* what) {
+        return E.cuda(E.dmalloc((void**) &p, sizeof(float) * floats), what) && E.cuda(E.dmemset(p, 0, sizeof(float) * floats), what);
+    }
+
+    template <class F> static void forEachSlotUse(const PendingOp& op, F&& f) {   // in operand order
+        for (auto& o : op.operands) if (o.first == K_SLOT) f(o.second);
+        for (auto& st : op.steps) if (!chain_fn_is_unary(st.fn) && st.kind == K_SLOT) f(st.ref);
+    }
+
+    // The values read in a later cut than the one that produced them, in order of first use (ring and buffer indices follow that
+    // order into the program words).  cut(s, i) is the cut (K1 stage, warp pipeline stage) of op i of segment s.
+    template <class Cut> static std::vector<int32_t> crossingValues(const Segments& segs, Cut cut) {
+        std::unordered_map<int32_t, int> producedIn;
+        for (size_t s = 0; s < segs.size(); ++s)
+            for (size_t i = 0; i < segs[s].size(); ++i) producedIn[segs[s][i].outNode] = cut(s, i);
+        std::vector<int32_t> crossing;
+        std::unordered_set<int32_t> seen;
+        for (size_t s = 0; s < segs.size(); ++s)
+            for (size_t i = 0; i < segs[s].size(); ++i)
+                forEachSlotUse(segs[s][i], [&](int32_t id) {
+                    auto p = producedIn.find(id);
+                    if (p != producedIn.end() && p->second < cut(s, i) && seen.insert(id).second) crossing.push_back(id);
+                });
+        return crossing;
+    }
+
+    // Slots by liveness, one linear scan over a section's ops in order: an op's output takes the slot freed last (or a new one) before
+    // its operands' slots are freed, so it never shares a slot with one of its own inputs; an operand's slot is freed after its last use
+    // in the section, operands in order, and an output nobody reads in the section at once.  Values in `ring` get no slot here.  Slots
+    // are numbered from `base`; returns how many were taken.
+    static int allocateSlots(Segments& section, const std::unordered_map<int32_t, int>& ring, int base) {
+        std::unordered_map<int32_t, size_t> lastUse;
+        size_t i = 0;
+        for (auto& ops : section)
+            for (auto& op : ops) { forEachSlotUse(op, [&](int32_t id) { lastUse[id] = i; }); ++i; }
+        std::unordered_map<int32_t, int> slotOf;
+        std::vector<int> freeSlots;
+        int n = 0;
+        i = 0;
+        for (auto& ops : section)
+            for (auto& op : ops) {
+                const bool inRing = ring.count(op.outNode) != 0;
+                if (!inRing) {
+                    int s = n;
+                    if (!freeSlots.empty()) { s = freeSlots.back(); freeSlots.pop_back(); }
+                    else ++n;
+                    op.slot = base + s;
+                    slotOf[op.outNode] = s;
+                }
+                forEachSlotUse(op, [&](int32_t id) {
+                    auto so = slotOf.find(id);
+                    if (so != slotOf.end() && lastUse[id] == i) { freeSlots.push_back(so->second); slotOf.erase(so); }
+                });
+                if (!inRing && !lastUse.count(op.outNode)) { freeSlots.push_back(op.slot - base); slotOf.erase(op.outNode); }
+                ++i;
+            }
+        return n;
+    }
 
     static void putDouble(PendingOp& op, double d) {
         uint64_t b;
@@ -1322,6 +1383,7 @@ struct Compiler {
 int Compiler::emitNode(Node& n, int rootIndex) {
     if (n.kind == NodeKind::Const || n.kind == NodeKind::Sr) return rc::Ok;   // folded into PARAM operands
 
+    std::vector<PendingOp>& ops = segs[(size_t) rootIndex];
     const bool leaf = n.inlets.empty();
     const bool sourceNode = n.kind == NodeKind::Rand || n.kind == NodeKind::TapIn || n.kind == NodeKind::Time || n.kind == NodeKind::Metro;
     if (leaf && !sourceNode) prog.usesHostInputs = true;
@@ -1451,8 +1513,7 @@ int Compiler::emitNode(Node& n, int rootIndex) {
             evNode = true;
             const size_t floats = (size_t) g.nTiles() * g.tileWidth * (size_t) n.size;
             if (!n.ring) {
-                if (!E.cuda(E.dmalloc((void**) &n.ring, sizeof(float) * floats), "cudaMalloc analysis ring")) return rc::CudaError;
-                if (!E.cuda(E.dmemset(n.ring, 0, sizeof(float) * floats), "memset analysis ring")) return rc::CudaError;
+                if (!zeroedFloats(n.ring, floats, "analysis ring")) return rc::CudaError;
                 n.ringFloats = floats;
             }
             if (n.kind == NodeKind::Scope || n.kind == NodeKind::Fft) {
@@ -1470,40 +1531,24 @@ int Compiler::emitNode(Node& n, int rootIndex) {
             op.ptr = (uint64_t) (uintptr_t) n.ring;
         } break;
 
-        case NodeKind::Delay: {   // Delays.h:92-106
-            const size_t tiles = (size_t) g.nTiles() * g.tileWidth;
+        case NodeKind::Delay:      // Delays.h:92-106
+        case NodeKind::SDelay: {   // Delays.h:221-245
             if (n.ringDirty) {
                 E.dsync();
                 if (n.ring) { E.dfree(n.ring); n.ring = nullptr; }
-                n.ringFloats = (size_t) n.size * tiles;
-                if (n.ringFloats) {
-                    if (!E.cuda(E.dmalloc((void**) &n.ring, sizeof(float) * n.ringFloats), "cudaMalloc delay ring")) return rc::CudaError;
-                    if (!E.cuda(E.dmemset(n.ring, 0, sizeof(float) * n.ringFloats), "memset ring")) return rc::CudaError;
-                }
+                n.ringFloats = (size_t) n.size * ((size_t) g.nTiles() * g.tileWidth);
+                if (n.ringFloats && !zeroedFloats(n.ring, n.ringFloats, "delay ring")) return rc::CudaError;
                 int r = E.fillRowBits(g, n.stateRow, 0, g.nv, 0);   // writeIndex = 0
                 if (r != rc::Ok) return r;
                 n.ringDirty = false;
             }
-            if (numCh < 3) { zeros(); break; }
-            op.opcode = OP_DELAY; op.aux0 = (uint32_t) n.size; op.ptr = (uint64_t) (uintptr_t) n.ring; take(3);
-        } break;
-
-        case NodeKind::SDelay: {  // Delays.h:221-245
-            const size_t tiles = (size_t) g.nTiles() * g.tileWidth;
-            if (n.ringDirty) {
-                E.dsync();
-                if (n.ring) { E.dfree(n.ring); n.ring = nullptr; }
-                n.ringFloats = (size_t) n.size * tiles;
-                if (n.ringFloats) {
-                    if (!E.cuda(E.dmalloc((void**) &n.ring, sizeof(float) * n.ringFloats), "cudaMalloc sdelay ring")) return rc::CudaError;
-                    if (!E.cuda(E.dmemset(n.ring, 0, sizeof(float) * n.ringFloats), "memset ring")) return rc::CudaError;
-                }
-                int r = E.fillRowBits(g, n.stateRow, 0, g.nv, 0);
-                if (r != rc::Ok) return r;
-                n.ringDirty = false;
+            if (n.kind == NodeKind::Delay) {
+                if (numCh < 3) { zeros(); break; }
+                op.opcode = OP_DELAY; op.aux0 = (uint32_t) n.size; op.ptr = (uint64_t) (uintptr_t) n.ring; take(3);
+            } else {
+                if (numCh < 1 || n.size == 0) { zeros(); break; }
+                op.opcode = OP_SDELAY; op.aux0 = (uint32_t) n.size; op.aux1 = (uint32_t) n.length; op.ptr = (uint64_t) (uintptr_t) n.ring; take(1);
             }
-            if (numCh < 1 || n.size == 0) { zeros(); break; }
-            op.opcode = OP_SDELAY; op.aux0 = (uint32_t) n.size; op.aux1 = (uint32_t) n.length; op.ptr = (uint64_t) (uintptr_t) n.ring; take(1);
         } break;
 
         case NodeKind::Table: {   // Table.h:44-57
@@ -1524,8 +1569,7 @@ int Compiler::emitNode(Node& n, int rootIndex) {
             if (!n.tapName.empty()) {   // Feedback.h:29-33: created on first request by either side
                 auto it = g.tapShared.find(n.tapName);
                 if (it == g.tapShared.end()) {
-                    if (!E.cuda(E.dmalloc((void**) &shared, sizeof(float) * floats), "cudaMalloc tap")) return rc::CudaError;
-                    if (!E.cuda(E.dmemset(shared, 0, sizeof(float) * floats), "memset tap")) return rc::CudaError;
+                    if (!zeroedFloats(shared, floats, "tap")) return rc::CudaError;
                     g.tapShared[n.tapName] = shared;
                 } else shared = it->second;
             }
@@ -1533,10 +1577,7 @@ int Compiler::emitNode(Node& n, int rootIndex) {
                 if (!shared) { zeros(); break; }
                 op.opcode = OP_TAPIN; op.ptr = (uint64_t) (uintptr_t) shared;
             } else {
-                if (!n.tapPrivate) {
-                    if (!E.cuda(E.dmalloc((void**) &n.tapPrivate, sizeof(float) * floats), "cudaMalloc tapOut")) return rc::CudaError;
-                    if (!E.cuda(E.dmemset(n.tapPrivate, 0, sizeof(float) * floats), "memset tapOut")) return rc::CudaError;
-                }
+                if (!n.tapPrivate && !zeroedFloats(n.tapPrivate, floats, "tapOut")) return rc::CudaError;
                 if (shared) promotes.push_back({rootIndex, n.id});
                 if (numCh < 1) { zeros(); break; }
                 op.opcode = OP_TAPOUT; op.ptr = (uint64_t) (uintptr_t) n.tapPrivate; take(1);
@@ -1553,7 +1594,7 @@ int Compiler::emitNode(Node& n, int rootIndex) {
                 n.conv = cs;
                 n.resourceDirty = false;
             }
-            op.opcode = 0xF0; take(1);   // OP_HOST_CONV: lowered to STOREBUF + K3 + LOADBUF by the stage pass
+            op.opcode = OP_HOST_CONV; take(1);
         } break;
 
         default: zeros(); break;
@@ -1589,28 +1630,21 @@ int Engine::compile(Group& g, int nIn, std::shared_ptr<Program>& out) {
         prog->rootIds.push_back(rid);
         std::vector<int32_t> order;
         traverse(g, visited, order, rid);
-        Compiler::PendingOp seg;
-        seg.isSeg = true; seg.opcode = OP_SEG; seg.segRoot = r; seg.segment = r;
-        const size_t segIdx = C.ops.size();
-        C.ops.push_back(seg);
+        C.segs.emplace_back();
         for (int32_t nid : order) {
             auto it = g.nodes.find(nid);
             if (it == g.nodes.end()) continue;
             prog->nodeIds.push_back(nid);
-            const size_t before = C.ops.size();
             int rcode = C.emitNode(it->second, r);
             if (rcode != rc::Ok) return rcode;
-            for (size_t k = before; k < C.ops.size(); ++k) C.ops[k].segment = r;
         }
-        C.ops[segIdx].segEndOp = C.ops.size();
     }
-    auto& ops = C.ops;
-    using Step = Compiler::PendingOp::Step;
-
-    auto forEachSlotUse = [](const Compiler::PendingOp& op, const std::function<void(int32_t)>& f) {
-        for (auto& o : op.operands) if (o.first == K_SLOT) f(o.second);
-        for (auto& st : op.steps) if (!chain_fn_is_unary(st.fn) && st.kind == K_SLOT) f(st.ref);
-    };
+    using PendingOp = Compiler::PendingOp;
+    using Segments = Compiler::Segments;
+    using Step = PendingOp::Step;
+    Segments& segs = C.segs;
+    bool hasConv = false;
+    for (auto& ops : segs) for (auto& op : ops) if (op.opcode == OP_HOST_CONV) hasConv = true;
 
     // ---- chain fusion -------------------------------------------------------------------------------------
     // An element-wise node whose output has exactly one use, by a later element-wise node of the same root
@@ -1620,263 +1654,215 @@ int Engine::compile(Group& g, int nIn, std::shared_ptr<Program>& out) {
     // same left-fold order (Math.h:71-84), so results are bit-identical; only the evaluation ORDER of
     // independent stateless nodes changes, and the intermediates stay in registers.
     if (opt_.fuseChains) {
-        std::unordered_map<int32_t, int> uses;
-        for (auto& op : ops) if (!op.isSeg) forEachSlotUse(op, [&](int32_t id) { ++uses[id]; });
-        std::unordered_map<int32_t, size_t> producer;   // value id -> index of the (still open) chain producing it
-        std::vector<Compiler::PendingOp> outOps;
-        std::vector<size_t> segHeaderAt(prog->rootIds.size(), 0);
-        int32_t& tempCounter = C.tempCounter;
-        for (size_t i = 0; i < ops.size(); ++i) {
-            Compiler::PendingOp op = ops[i];
-            if (op.isSeg) { segHeaderAt[op.segRoot] = outOps.size(); outOps.push_back(op); continue; }
-            if (op.opcode != OP_CHAIN) { outOps.push_back(op); continue; }
-            auto absorbable = [&](uint32_t kind, int32_t ref) -> long {
-                if (kind != K_SLOT) return -1;
-                auto u = uses.find(ref);
-                if (u == uses.end() || u->second != 1) return -1;
-                auto p = producer.find(ref);
-                if (p == producer.end()) return -1;
-                const auto& pop = outOps[p->second];
-                if (pop.dead || pop.opcode != OP_CHAIN || pop.segment != op.segment) return -1;
-                return (long) p->second;
-            };
-            // head: the first operand's producer continues into this chain
-            Compiler::PendingOp cur = op;
-            cur.steps.clear();
-            {
-                long pi = absorbable(op.operands[0].first, op.operands[0].second);
-                if (pi >= 0) {
+        std::unordered_map<int32_t, int> uses;   // over the whole program: a value read once, but by another root's op, stays
+        for (auto& ops : segs) for (auto& op : ops) Compiler::forEachSlotUse(op, [&](int32_t id) { ++uses[id]; });
+        for (auto& ops : segs) {
+            std::unordered_map<int32_t, size_t> producer;   // value id -> index of the (still open) chain producing it in this segment
+            std::vector<PendingOp> outOps;
+            for (PendingOp& op : ops) {
+                if (op.opcode != OP_CHAIN) { outOps.push_back(std::move(op)); continue; }
+                auto absorbable = [&](uint32_t kind, int32_t ref) -> long {
+                    if (kind != K_SLOT) return -1;
+                    auto u = uses.find(ref);
+                    if (u == uses.end() || u->second != 1) return -1;
+                    auto p = producer.find(ref);
+                    if (p == producer.end()) return -1;
+                    const auto& pop = outOps[p->second];
+                    if (pop.dead || pop.opcode != OP_CHAIN) return -1;
+                    return (long) p->second;
+                };
+                // head: the first operand's producer continues into this chain
+                PendingOp cur = op;
+                cur.steps.clear();
+                {
+                    long pi = absorbable(op.operands[0].first, op.operands[0].second);
+                    if (pi >= 0) {
+                        cur.operands = outOps[pi].operands;
+                        cur.steps = outOps[pi].steps;
+                        outOps[pi].dead = true;
+                    }
+                }
+                for (const Step& st : op.steps) {
+                    long pi = chain_fn_is_unary(st.fn) ? -1 : absorbable(st.kind, st.ref);
+                    if (pi < 0 || cur.steps.size() + outOps[pi].steps.size() > 200) { cur.steps.push_back(st); continue; }
+                    // flush the running value to a temporary, then restart from the absorbed producer and finish
+                    // with the reversed step: value = fn(running, producer)
+                    uint32_t runKind = cur.operands[0].first;
+                    int32_t runRef = cur.operands[0].second;
+                    if (!cur.steps.empty()) {
+                        PendingOp flushed = cur;
+                        flushed.outNode = C.newTemp();
+                        flushed.state = NO_STATE;
+                        outOps.push_back(flushed);
+                        runKind = K_SLOT; runRef = flushed.outNode;
+                    }
                     cur.operands = outOps[pi].operands;
                     cur.steps = outOps[pi].steps;
                     outOps[pi].dead = true;
+                    cur.steps.push_back({st.fn | CHAIN_REVERSED, runKind, runRef});
                 }
-            }
-            for (const Step& st : op.steps) {
-                long pi = chain_fn_is_unary(st.fn) ? -1 : absorbable(st.kind, st.ref);
-                if (pi < 0 || cur.steps.size() + outOps[pi].steps.size() > 200) { cur.steps.push_back(st); continue; }
-                // flush the running value to a temporary, then restart from the absorbed producer and finish
-                // with the reversed step: value = fn(running, producer)
-                uint32_t runKind = cur.operands[0].first;
-                int32_t runRef = cur.operands[0].second;
-                if (!cur.steps.empty()) {
-                    Compiler::PendingOp flushed = cur;
-                    flushed.outNode = INT32_MIN + (++tempCounter);
-                    flushed.state = NO_STATE;
-                    outOps.push_back(flushed);
-                    runKind = K_SLOT; runRef = flushed.outNode;
-                }
-                cur.operands = outOps[pi].operands;
-                cur.steps = outOps[pi].steps;
-                outOps[pi].dead = true;
-                cur.steps.push_back({st.fn | CHAIN_REVERSED, runKind, runRef});
-            }
-            if (cur.steps.size() > 120) {   // keep every op's operand block within 255 words
-                // split: flush the first 100 steps into a temporary and continue from it
+                // keep every op's operand block within 255 words: flush the first 100 steps into a temporary and continue from it
                 while (cur.steps.size() > 120) {
-                    Compiler::PendingOp head = cur;
+                    PendingOp head = cur;
                     head.steps.assign(cur.steps.begin(), cur.steps.begin() + 100);
-                    head.outNode = INT32_MIN + (++tempCounter);
+                    head.outNode = C.newTemp();
                     outOps.push_back(head);
                     cur.operands = {{K_SLOT, head.outNode}};
                     cur.steps.erase(cur.steps.begin(), cur.steps.begin() + 100);
                 }
+                producer[cur.outNode] = outOps.size();
+                outOps.push_back(std::move(cur));
             }
-            producer[cur.outNode] = outOps.size();
-            outOps.push_back(cur);
+            ops.clear();   // drop absorbed ops
+            for (auto& op : outOps) if (!op.dead) ops.push_back(std::move(op));
         }
-        // drop absorbed ops, fix segment ends
-        std::vector<Compiler::PendingOp> compact;
-        std::vector<size_t> segStart(prog->rootIds.size(), 0);
-        for (auto& op : outOps) {
-            if (op.dead) continue;
-            if (op.isSeg) segStart[op.segRoot] = compact.size();
-            compact.push_back(op);
-        }
-        for (size_t r = 0; r < segStart.size(); ++r) {
-            size_t end = compact.size();
-            for (size_t k = segStart[r] + 1; k < compact.size(); ++k) if (compact[k].isSeg) { end = k; break; }
-            compact[segStart[r]].segEndOp = end;
-        }
-        ops.swap(compact);
 
         // ---- re-schedule each root sub-sequence to shorten live ranges -----------------------------------------
         // Depth-first from the sinks of the segment, visiting the operand with the larger sub-tree first
         // (Sethi-Ullman order).  Any topological order gives the same results — every op is a function of its
         // operand values and its own private state only — but this one keeps a 64-partial additive voice at 3
         // live slots instead of 65.
-        std::vector<Compiler::PendingOp> sched;
-        size_t i0 = 0;
-        while (i0 < ops.size()) {
-            const size_t segBegin = i0;                       // ops[segBegin] is the OP_SEG header
-            const size_t segEnd = ops[segBegin].segEndOp;
+        for (auto& ops : segs) {
+            const size_t n = ops.size();
             std::unordered_map<int32_t, size_t> prodIdx;      // value id -> op index inside this segment
-            for (size_t k = segBegin + 1; k < segEnd; ++k) prodIdx[ops[k].outNode] = k;
-            std::vector<std::vector<size_t>> deps(segEnd - segBegin);
-            std::vector<int> consumers(segEnd - segBegin, 0);
-            for (size_t k = segBegin + 1; k < segEnd; ++k)
-                forEachSlotUse(ops[k], [&](int32_t id) {
+            for (size_t k = 0; k < n; ++k) prodIdx[ops[k].outNode] = k;
+            std::vector<std::vector<size_t>> deps(n);
+            std::vector<int> consumers(n, 0);
+            for (size_t k = 0; k < n; ++k)
+                Compiler::forEachSlotUse(ops[k], [&](int32_t id) {
                     auto p = prodIdx.find(id);
-                    if (p != prodIdx.end() && p->second != k) { deps[k - segBegin].push_back(p->second); ++consumers[p->second - segBegin]; }
+                    if (p != prodIdx.end() && p->second != k) { deps[k].push_back(p->second); ++consumers[p->second]; }
                 });
-            std::vector<long> weight(segEnd - segBegin, -1);
+            std::vector<long> weight(n, -1);
             std::function<long(size_t)> subtree = [&](size_t k) -> long {
-                long& w = weight[k - segBegin];
+                long& w = weight[k];
                 if (w >= 0) return w;
                 w = 1;
-                for (size_t d : deps[k - segBegin]) w += subtree(d);
+                for (size_t d : deps[k]) w += subtree(d);
                 return w;
             };
-            std::vector<char> done(segEnd - segBegin, 0);
-            const size_t headerAt = sched.size();
-            sched.push_back(ops[segBegin]);
+            std::vector<char> done(n, 0);
+            std::vector<PendingOp> sched;
             std::function<void(size_t)> emit = [&](size_t k) {
-                if (done[k - segBegin]) return;
-                done[k - segBegin] = 1;
-                std::vector<size_t> ds = deps[k - segBegin];
+                if (done[k]) return;
+                done[k] = 1;
+                std::vector<size_t> ds = deps[k];
                 std::stable_sort(ds.begin(), ds.end(), [&](size_t a, size_t b) { return subtree(a) > subtree(b); });
                 for (size_t d : ds) emit(d);
-                sched.push_back(ops[k]);
+                sched.push_back(std::move(ops[k]));
             };
-            for (size_t k = segBegin + 1; k < segEnd; ++k) if (consumers[k - segBegin] == 0) emit(k);
-            for (size_t k = segBegin + 1; k < segEnd; ++k) emit(k);   // anything unreachable (cannot happen) keeps its place
-            sched[headerAt].segEndOp = sched.size();
-            i0 = segEnd;
+            for (size_t k = 0; k < n; ++k) if (consumers[k] == 0) emit(k);
+            for (size_t k = 0; k < n; ++k) emit(k);   // anything unreachable (cannot happen) keeps its place
+            ops.swap(sched);
         }
-        ops.swap(sched);
 
         // ---- group independent constant-frequency phasors into runs ----------------------------------------------
         // A phasor fed by a parameter depends on nothing, so it may run anywhere in its segment.  With L < 32 voices
         // per warp only L lanes work in a recurrence; a run of R <= 32/L such phasors is executed by R lane groups
         // in one serial loop (render_kernel.cu, OP_PHASOR with aux1 = R).  Followers are pulled forward to sit
-        // right behind the leader; the look-ahead is bounded so live ranges stay short.
-        bool staged = false;   // programs cut into stages (convolve) insert spill ops between ops: keep them ungrouped
-        for (auto& op : ops) if (op.opcode == 0xF0) staged = true;
-        const int maxRun = staged ? 1 : std::min(8, 32 / std::max(1, g.tileWidth));
-        auto isParamPhasor = [](const Compiler::PendingOp& op) {
-            return !op.isSeg && op.opcode == OP_PHASOR && op.operands.size() == 1 && op.operands[0].first != K_SLOT;
+        // right behind the leader; the look-ahead is bounded so live ranges stay short.  Programs cut into stages
+        // (convolve) insert spill ops between ops: they keep their phasors ungrouped.
+        const int maxRun = hasConv ? 1 : std::min(8, 32 / std::max(1, g.tileWidth));
+        auto isParamPhasor = [](const PendingOp& op) {
+            return op.opcode == OP_PHASOR && op.operands.size() == 1 && op.operands[0].first != K_SLOT;
         };
-        for (size_t i = 0; i < ops.size(); ++i) {
-            if (!isParamPhasor(ops[i]) || ops[i].aux1 != 0 || ops[i].mode == 1) continue;
-            size_t segEnd = ops.size();
-            for (size_t k = i + 1; k < ops.size(); ++k) if (ops[k].isSeg) { segEnd = k; break; }
-            uint32_t run = 1;
-            for (size_t j = i + 1; j < segEnd && j < i + 1 + (size_t) 4 * maxRun && (int) run < maxRun; ++j) {
-                if (!isParamPhasor(ops[j]) || ops[j].mode == 1) continue;
-                Compiler::PendingOp follower = ops[j];
-                follower.mode = 1;                     // marks "member of a run" (never dispatched on its own)
-                ops.erase(ops.begin() + (long) j);
-                ops.insert(ops.begin() + (long) (i + run), follower);
-                ++run;
+        for (auto& ops : segs)
+            for (size_t i = 0; i < ops.size(); ++i) {
+                if (!isParamPhasor(ops[i]) || ops[i].aux1 != 0 || ops[i].mode == 1) continue;
+                uint32_t run = 1;
+                for (size_t j = i + 1; j < ops.size() && j < i + 1 + (size_t) 4 * maxRun && (int) run < maxRun; ++j) {
+                    if (!isParamPhasor(ops[j]) || ops[j].mode == 1) continue;
+                    PendingOp follower = ops[j];
+                    follower.mode = 1;                     // marks "member of a run" (never dispatched on its own)
+                    ops.erase(ops.begin() + (long) j);
+                    ops.insert(ops.begin() + (long) (i + run), follower);
+                    ++run;
+                }
+                ops[i].aux1 = run;                         // run length, 1 = a lone constant-frequency phasor
             }
-            ops[i].aux1 = run;                         // run length, 1 = a lone constant-frequency phasor
-        }
     }
 
     // ---- stages: a `convolve` node is a whole-block operation (K3) that cannot live inside the sample-tiled
     // interpreter, so the program is cut into K1 stages around it.  Values that cross a stage boundary travel
     // through per-voice block buffers in HBM (OP_STOREBUF / OP_LOADBUF); root ops always run in the last stage.
-    constexpr uint32_t OP_HOST_CONV = 0xF0;   // host-only pseudo opcode emitted for Convolve nodes
-    std::vector<std::vector<Compiler::PendingOp>> stageOps;
-    bool hasConv = false;
-    for (auto& op : ops) if (op.opcode == OP_HOST_CONV) hasConv = true;
+    std::vector<Segments> stageOps;   // per K1 stage, one op list per root
     if (!hasConv) {
-        stageOps.push_back(ops);
+        stageOps.push_back(std::move(segs));
     } else {
         std::unordered_map<int32_t, int> stageOfValue;       // stage in which the value becomes available to K1
-        std::unordered_map<int32_t, const Compiler::PendingOp*> producerOp;
+        std::vector<std::vector<int>> stageOfOp(segs.size());
         int lastStage = 0;
-        std::vector<int> stageOfOp(ops.size(), 0);
-        for (size_t i = 0; i < ops.size(); ++i) {
-            auto& op = ops[i];
-            if (op.isSeg) continue;
-            int st = 0;
-            forEachSlotUse(op, [&](int32_t id) { auto it = stageOfValue.find(id); if (it != stageOfValue.end()) st = std::max(st, it->second); });
-            stageOfOp[i] = st;
-            stageOfValue[op.outNode] = (op.opcode == OP_HOST_CONV) ? st + 1 : st;
-            lastStage = std::max(lastStage, stageOfValue[op.outNode]);
-        }
-        for (size_t i = 0; i < ops.size(); ++i) if (!ops[i].isSeg && ops[i].opcode == OP_ROOT) stageOfOp[i] = lastStage;
+        for (size_t s = 0; s < segs.size(); ++s)
+            for (auto& op : segs[s]) {
+                int st = 0;
+                Compiler::forEachSlotUse(op, [&](int32_t id) { auto it = stageOfValue.find(id); if (it != stageOfValue.end()) st = std::max(st, it->second); });
+                stageOfOp[s].push_back(st);
+                stageOfValue[op.outNode] = (op.opcode == OP_HOST_CONV) ? st + 1 : st;
+                lastStage = std::max(lastStage, stageOfValue[op.outNode]);
+            }
+        for (size_t s = 0; s < segs.size(); ++s)
+            for (size_t i = 0; i < segs[s].size(); ++i) if (segs[s][i].opcode == OP_ROOT) stageOfOp[s][i] = lastStage;
         const int nStages = lastStage + 1;
         const size_t blockFloats = (size_t) g.Vpad * blockSize_;
         auto newBlockBuffer = [&]() -> float* {
             float* p = nullptr;
-            if (!cuda(dmalloc((void**) &p, sizeof(float) * blockFloats), "cudaMalloc stage buffer")) return nullptr;
-            dmemset(p, 0, sizeof(float) * blockFloats);
-            prog->blockBuffers.push_back(p);
-            return p;
+            const bool ok = C.zeroedFloats(p, blockFloats, "stage buffer");
+            if (p) prog->blockBuffers.push_back(p);   // freed with the program
+            return ok ? p : nullptr;
         };
         // buffers: one per convolve node (in, out) and one per ordinary value that crosses stages
         std::unordered_map<int32_t, float*> spillOf;         // value id -> HBM block buffer holding it
+        std::unordered_set<int32_t> bypassed;                // host input values convolvers read where they lie
         prog->stages.resize(nStages);
-        for (size_t i = 0; i < ops.size(); ++i) {
-            auto& op = ops[i];
-            if (op.isSeg || op.opcode != OP_HOST_CONV) continue;
-            Node& n = g.nodes.at(op.outNode);
-            // A convolver fed straight by a host input channel (`convolve(in)`) reads that channel where it lies: no K1 staging
-            // copy, and — when nothing else lives in the stage — no K1 launch at all for it.
-            int inChannel = -1;
-            if (op.operands.size() == 1 && op.operands[0].first == K_SLOT) {
-                for (size_t j = 0; j < i; ++j)
-                    if (!ops[j].isSeg && ops[j].outNode == op.operands[0].second && ops[j].opcode == OP_LOADIN) inChannel = (int) ops[j].aux0;
+        for (size_t s = 0; s < segs.size(); ++s)
+            for (size_t i = 0; i < segs[s].size(); ++i) {
+                auto& op = segs[s][i];
+                if (op.opcode != OP_HOST_CONV) continue;
+                Node& n = g.nodes.at(op.outNode);
+                // A convolver fed straight by a host input channel (`convolve(in)`) reads that channel where it lies: no K1 staging
+                // copy, and — when nothing else lives in the stage — no K1 launch at all for it.
+                int inChannel = -1;
+                if (op.operands.size() == 1 && op.operands[0].first == K_SLOT)
+                    for (auto& ops : segs)
+                        for (auto& ld : ops) if (ld.outNode == op.operands[0].second && ld.opcode == OP_LOADIN) inChannel = (int) ld.aux0;
+                float* inB = inChannel >= 0 ? nullptr : newBlockBuffer();
+                float* outB = newBlockBuffer();
+                if ((inChannel < 0 && !inB) || !outB) return rc::CudaError;
+                prog->stages[stageOfOp[s][i]].convolves.push_back({n.id, inB, outB, inChannel});
+                spillOf[op.outNode] = outB;
+                op.ptr = (uint64_t) (uintptr_t) inB;
+                if (inChannel >= 0) { op.mode = 1; bypassed.insert(op.operands[0].second); }   // mode 1: no STOREBUF needed
             }
-            float* inB = inChannel >= 0 ? nullptr : newBlockBuffer();
-            float* outB = newBlockBuffer();
-            if ((inChannel < 0 && !inB) || !outB) return rc::CudaError;
-            prog->stages[stageOfOp[i]].convolves.push_back({n.id, inB, outB, inChannel});
-            spillOf[op.outNode] = outB;
-            op.ptr = (uint64_t) (uintptr_t) inB;
-            if (inChannel >= 0) op.mode = 1;      // marks "no STOREBUF needed"
-        }
         // LOADINs whose only consumers are bypassed convolvers are dead
-        {
-            std::unordered_map<int32_t, int> otherUses;
-            for (auto& op : ops) {
-                if (op.isSeg || (op.opcode == OP_HOST_CONV && op.mode == 1)) continue;
-                forEachSlotUse(op, [&](int32_t id) { ++otherUses[id]; });
-            }
-            for (auto& op : ops)
-                if (!op.isSeg && op.opcode == OP_LOADIN && !otherUses.count(op.outNode)) {
-                    bool feedsBypass = false;
-                    for (auto& c : ops) if (!c.isSeg && c.opcode == OP_HOST_CONV && c.mode == 1 && c.operands[0].second == op.outNode) feedsBypass = true;
-                    if (feedsBypass) op.dead = true;
-                }
-        }
-        // which values are read in a later stage than the one that produces them?
-        std::unordered_map<int32_t, int> producedIn;
-        for (size_t i = 0; i < ops.size(); ++i) if (!ops[i].isSeg) producedIn[ops[i].outNode] = (ops[i].opcode == OP_HOST_CONV) ? -1 : stageOfOp[i];
-        for (size_t i = 0; i < ops.size(); ++i) {
-            if (ops[i].isSeg) continue;
-            forEachSlotUse(ops[i], [&](int32_t id) {
-                auto p = producedIn.find(id);
-                if (p == producedIn.end() || p->second < 0) return;
-                if (p->second < stageOfOp[i] && !spillOf.count(id)) spillOf[id] = nullptr;   // allocate below
-            });
-        }
-        for (auto& kv : spillOf) if (!kv.second) { kv.second = newBlockBuffer(); if (!kv.second) return rc::CudaError; }
+        std::unordered_set<int32_t> otherUses;
+        for (auto& ops : segs)
+            for (auto& op : ops) if (!(op.opcode == OP_HOST_CONV && op.mode == 1)) Compiler::forEachSlotUse(op, [&](int32_t id) { otherUses.insert(id); });
+        for (auto& ops : segs)
+            for (auto& op : ops) if (op.opcode == OP_LOADIN && bypassed.count(op.outNode) && !otherUses.count(op.outNode)) op.dead = true;
+        // convolver outputs already have their buffer
+        for (int32_t id : Compiler::crossingValues(segs, [&](size_t s, size_t i) { return stageOfOp[s][i]; }))
+            if (!spillOf.count(id) && !(spillOf[id] = newBlockBuffer())) return rc::CudaError;
 
-        stageOps.assign(nStages, {});
+        stageOps.assign(nStages, Segments(segs.size()));
         for (int st = 0; st < nStages; ++st) {
-            auto& out = stageOps[st];
-            size_t i = 0;
-            while (i < ops.size()) {
-                const size_t segBegin = i, segEnd = ops[i].segEndOp;
-                const size_t headerAt = out.size();
-                out.push_back(ops[segBegin]);
+            bool anyWork = false;
+            std::unordered_set<int32_t> producedHere;
+            for (size_t s = 0; s < segs.size(); ++s) {
+                auto& out = stageOps[st][s];
                 std::unordered_map<int32_t, int32_t> loaded;   // value id -> temp id loaded in this stage+segment
-                for (size_t k = segBegin + 1; k < segEnd; ++k) {
-                    if (stageOfOp[k] != st || ops[k].dead) continue;
-                    Compiler::PendingOp op = ops[k];
+                for (size_t i = 0; i < segs[s].size(); ++i) {
+                    if (stageOfOp[s][i] != st || segs[s][i].dead) continue;
+                    PendingOp op = segs[s][i];
                     // reload operands that were produced in an earlier stage (or by a convolver)
                     auto fix = [&](uint32_t& kind, int32_t& ref) {
-                        if (kind != K_SLOT) return;
-                        auto p = producedIn.find(ref);
-                        if (p == producedIn.end()) return;
-                        if (p->second >= 0 && p->second >= st) return;
+                        if (kind != K_SLOT || producedHere.count(ref)) return;
+                        auto sp = spillOf.find(ref);
+                        if (sp == spillOf.end()) return;
                         auto l = loaded.find(ref);
                         if (l == loaded.end()) {
-                            Compiler::PendingOp ld;
-                            ld.opcode = OP_LOADBUF; ld.segment = op.segment; ld.outNode = INT32_MIN + (++C.tempCounter);
-                            ld.ptr = (uint64_t) (uintptr_t) spillOf.at(ref);
+                            PendingOp ld;
+                            ld.opcode = OP_LOADBUF; ld.outNode = C.newTemp();
+                            ld.ptr = (uint64_t) (uintptr_t) sp->second;
                             out.push_back(ld);
                             l = loaded.emplace(ref, ld.outNode).first;
                         }
@@ -1886,38 +1872,34 @@ int Engine::compile(Group& g, int nIn, std::shared_ptr<Program>& out) {
                     for (auto& stp : op.steps) if (!chain_fn_is_unary(stp.fn)) fix(stp.kind, stp.ref);
                     if (op.opcode == OP_HOST_CONV && op.mode == 1) continue;   // reads the host input channel directly
                     if (op.opcode == OP_HOST_CONV) {          // stage the convolver input
-                        op.opcode = OP_STOREBUF; op.state = NO_STATE; op.outNode = INT32_MIN + (++C.tempCounter);
+                        op.opcode = OP_STOREBUF; op.state = NO_STATE; op.outNode = C.newTemp();
                         out.push_back(op);
                         continue;
                     }
                     out.push_back(op);
+                    producedHere.insert(op.outNode);
                     auto sp = spillOf.find(op.outNode);
                     if (sp != spillOf.end()) {                // the value is needed by a later stage
-                        Compiler::PendingOp stb;
-                        stb.opcode = OP_STOREBUF; stb.segment = op.segment; stb.outNode = INT32_MIN + (++C.tempCounter);
+                        PendingOp stb;
+                        stb.opcode = OP_STOREBUF; stb.outNode = C.newTemp();
                         stb.operands = {{K_SLOT, op.outNode}};
                         stb.ptr = (uint64_t) (uintptr_t) sp->second;
                         out.push_back(stb);
                     }
                 }
-                out[headerAt].segEndOp = out.size();
-                i = segEnd;
+                anyWork = anyWork || !out.empty();
             }
-            bool anyWork = false;
-            for (auto& op : out) if (!op.isSeg) anyWork = true;
             prog->stages[st].empty = !anyWork;
         }
         // `convolve -> root` (a reverb send, BASELINE config 4): the last stage is [LOADBUF conv.out][ROOT of it] and nothing else
         if (opt_.fuseConvRoot && g.tileWidth == 1 && nStages >= 2 && prog->rootIds.size() == 1 && C.promotes.empty()) {
-            const auto& lastOps = stageOps[nStages - 1];
-            std::vector<const Compiler::PendingOp*> body;
-            for (auto& op : lastOps) if (!op.isSeg) body.push_back(&op);
-            if (body.size() == 2 && body[0]->opcode == OP_LOADBUF && body[1]->opcode == OP_ROOT && body[1]->operands.size() == 1 &&
-                body[1]->operands[0].first == K_SLOT && body[1]->operands[0].second == body[0]->outNode) {
+            const auto& body = stageOps[nStages - 1][0];
+            if (body.size() == 2 && body[0].opcode == OP_LOADBUF && body[1].opcode == OP_ROOT && body[1].operands.size() == 1 &&
+                body[1].operands[0].first == K_SLOT && body[1].operands[0].second == body[0].outNode) {
                 for (int st = 0; st < nStages - 1 && prog->fusedConvStage < 0; ++st)
                     for (size_t ci = 0; ci < prog->stages[st].convolves.size(); ++ci)
-                        if ((uint64_t) (uintptr_t) prog->stages[st].convolves[ci].out == body[0]->ptr) {
-                            prog->fusedConvStage = st; prog->fusedConvIndex = (int) ci; prog->fusedRoot = (int) body[1]->aux0;
+                        if ((uint64_t) (uintptr_t) prog->stages[st].convolves[ci].out == body[0].ptr) {
+                            prog->fusedConvStage = st; prog->fusedConvIndex = (int) ci; prog->fusedRoot = (int) body[1].aux0;
                             break;
                         }
             }
@@ -1930,15 +1912,16 @@ int Engine::compile(Group& g, int nIn, std::shared_ptr<Program>& out) {
     // own warp, and the warps work on consecutive sample tiles of the same graph at the same time.  A value that crosses a cut lives in
     // a ring slot with W buffers (tile index mod W), everything else in slots private to its stage.  Same ops, same order of evaluation
     // per value: bit-identical output (tests/test_parity_gpu.py::test_pipelined_groups_equal_the_unpipelined_path).
-    std::vector<int> pipeStageOf;            // per op of stageOps[0]; empty = not pipelined
+    std::vector<int> pipeStageOf;            // per op of the one segment of stageOps[0]; empty = not pipelined
     {
         const bool batchedGroup = groups_.size() > 1 && opt_.batchGroups;
         int W = std::min(opt_.pipelineStages, (int) MAX_PIPE);
         bool ok = W > 1 && batchedGroup && g.tileWidth == 1 && stageOps.size() == 1 && prog->rootIds.size() == 1 && C.promotes.empty() &&
                   prog->evNodes.empty() && prog->dynNodes.empty() && !prog->hasCustom;
-        auto& sops = stageOps[0];
-        auto costOf = [](const Compiler::PendingOp& op) -> long {     // cycles of one 32-sample tile at L = 1, dispatch included: measured per
-            switch (op.opcode) {                                          // opcode with the cycle-counter build (-DEB_OPPROF)
+        // cycles of one 32-sample tile at L = 1, dispatch included: measured per opcode with the cycle-counter build (-DEB_OPPROF);
+        // -1: an op the pipeline does not take
+        auto costOf = [](const PendingOp& op) -> long {
+            switch (op.opcode) {
                 case OP_CHAIN: {
                     long c = 350;
                     for (auto& st : op.steps) {
@@ -1965,26 +1948,18 @@ int Engine::compile(Group& g, int nIn, std::shared_ptr<Program>& out) {
                 case OP_SDELAY: case OP_TABLE: return 800;
                 case OP_Z: return 700;
                 case OP_ROOT: return 1100;
-                default: return 300;
+                case OP_FILL0: case OP_COPY: return 300;
+                default: return -1;
             }
         };
+        if (ok)
+            for (auto& op : stageOps[0][0]) ok = ok && costOf(op) >= 0;
         if (ok) {
-            for (size_t i = 0; i < sops.size() && ok; ++i) {
-                const auto& op = sops[i];
-                if (op.isSeg) { ok = (i == 0); continue; }
-                switch (op.opcode) {
-                    case OP_FILL0: case OP_COPY: case OP_CHAIN: case OP_PHASOR: case OP_SPHASOR: case OP_COUNTER: case OP_ACCUM: case OP_LATCH:
-                    case OP_MAXHOLD: case OP_RAND: case OP_POLE: case OP_ENV: case OP_BIQUAD: case OP_PREWARP: case OP_MM1P: case OP_SVF:
-                    case OP_SVFSHELF: case OP_Z: case OP_DELAY: case OP_SDELAY: case OP_TABLE: case OP_BLEP: case OP_ROOT: break;
-                    default: ok = false;
-                }
-            }
-        }
-        if (ok) {
+            const auto& sops = stageOps[0][0];
             // units: an op, or a phasor run (leader + its followers), which must stay together
             std::vector<std::pair<size_t, size_t>> units;     // [first op, one past the last op)
             std::vector<long> ucost;
-            for (size_t i = 1; i < sops.size();) {
+            for (size_t i = 0; i < sops.size();) {
                 size_t j = i + 1;
                 if (sops[i].opcode == OP_PHASOR && sops[i].aux1 > 1) j = i + sops[i].aux1;
                 long c = 0;
@@ -1994,8 +1969,7 @@ int Engine::compile(Group& g, int nIn, std::shared_ptr<Program>& out) {
                 i = j;
             }
             const int n = (int) units.size();
-            if (n < 2 * W) ok = false;
-            if (ok) {
+            if (n >= 2 * W) {
                 // linear partition: minimise the most expensive stage (O(n^2 W), n <= a few hundred)
                 std::vector<long> pre(n + 1, 0);
                 for (int i = 0; i < n; ++i) pre[i + 1] = pre[i] + ucost[i];
@@ -2017,15 +1991,14 @@ int Engine::compile(Group& g, int nIn, std::shared_ptr<Program>& out) {
                 for (int w = 0; w < W; ++w)
                     for (int u = bounds[w]; u < bounds[w + 1]; ++u)
                         for (size_t k = units[u].first; k < units[u].second; ++k) pipeStageOf[k] = w;
-                for (size_t i = 1; i < sops.size(); ++i)          // roots write the graph's output accumulator: last stage only
+                for (size_t i = 0; i < sops.size(); ++i)          // roots write the graph's output accumulator: last stage only
                     if (sops[i].opcode == OP_ROOT && pipeStageOf[i] != W - 1) { pipeStageOf.clear(); break; }
                 if (!pipeStageOf.empty()) { prog->pipeW = W; prog->pipeDepth = W; }
             }
         }
     }
 
-    // ---- per stage: slot allocation by liveness (an output slot is never the slot of one of its own inputs),
-    //      then encoding ----
+    // ---- per stage: slot allocation by liveness, then encoding ----
     std::unordered_map<uint32_t, uint32_t> smemIndexOfRow;
     int nStateRows = 0;
     auto mapState = [&](Node& n) -> uint32_t {
@@ -2048,104 +2021,49 @@ int Engine::compile(Group& g, int nIn, std::shared_ptr<Program>& out) {
         return idx;
     };
     std::unordered_map<int32_t, uint32_t> smemParamOfRow;
+    auto emitEnd = [&]() { for (int k = 0; k < 8; ++k) prog->code.push_back(k == 0 ? make_w0(OP_END, 0, 0, 0) : 0u); };
     int nSlotsMax = 1;
     prog->nOps = 0;
     if (prog->stages.empty()) prog->stages.resize(1);
     for (size_t stg = 0; stg < stageOps.size(); ++stg) {
-        auto& sops = stageOps[stg];
         prog->stages[stg].codeOffset = (uint32_t) prog->code.size();
 
-        std::vector<int> outSlot(sops.size(), 0);
+        // the sections K1 walks: the stage, or one per pipeline stage, each [SEG header][ops] per root
+        std::vector<Segments> sections;
         int nSlots = 0;
-        bool piped = !pipeStageOf.empty() && stg == 0;
-        if (piped) {
-            // ring values: read in a later pipeline stage than the one that produces them
-            const int W = prog->pipeW;
-            std::unordered_map<int32_t, int> prodStage, ringOf;
-            for (size_t i = 0; i < sops.size(); ++i) if (!sops[i].isSeg) prodStage[sops[i].outNode] = pipeStageOf[i];
-            int nRing = 0;
-            for (size_t i = 0; i < sops.size(); ++i) {
-                if (sops[i].isSeg) continue;
-                forEachSlotUse(sops[i], [&](int32_t id) {
-                    auto ps = prodStage.find(id);
-                    if (ps != prodStage.end() && ps->second < pipeStageOf[i] && !ringOf.count(id)) ringOf[id] = nRing++;
-                });
-            }
-            // private slots: liveness inside each stage, every stage in its own index range
-            int privBase = 0;
-            for (int w = 0; w < W; ++w) {
-                std::unordered_map<int32_t, size_t> lastUse;
-                for (size_t i = 0; i < sops.size(); ++i)
-                    if (!sops[i].isSeg && pipeStageOf[i] == w) forEachSlotUse(sops[i], [&](int32_t id) { lastUse[id] = i; });
-                std::unordered_map<int32_t, int> slotOf;
-                std::vector<int> freeSlots;
-                int local = 0;
-                for (size_t i = 0; i < sops.size(); ++i) {
-                    auto& op = sops[i];
-                    if (op.isSeg || pipeStageOf[i] != w) continue;
-                    auto rg = ringOf.find(op.outNode);
-                    if (rg != ringOf.end()) {
-                        outSlot[i] = -(rg->second + 1);                      // placed behind the private ranges below
-                    } else {
-                        int sl;
-                        if (!freeSlots.empty()) { sl = freeSlots.back(); freeSlots.pop_back(); }
-                        else sl = local++;
-                        outSlot[i] = privBase + sl;
-                        slotOf[op.outNode] = sl;
-                    }
-                    forEachSlotUse(op, [&](int32_t id) {
-                        auto lu = lastUse.find(id);
-                        auto so = slotOf.find(id);
-                        if (lu != lastUse.end() && lu->second == i && so != slotOf.end()) { freeSlots.push_back(so->second); slotOf.erase(so); }
-                    });
-                    if (rg == ringOf.end() && !lastUse.count(op.outNode)) {
-                        auto so = slotOf.find(op.outNode);
-                        if (so != slotOf.end()) { freeSlots.push_back(so->second); slotOf.erase(so); }
-                    }
-                }
-                privBase += local;
-            }
+        if (stg == 0 && !pipeStageOf.empty()) {
+            const auto& sops = stageOps[0][0];
+            std::unordered_map<int32_t, int> ringOf;   // ring values: read in a later pipeline stage than the one that produces them
+            for (int32_t id : Compiler::crossingValues(stageOps[0], [&](size_t, size_t i) { return pipeStageOf[i]; }))
+                ringOf.emplace(id, (int) ringOf.size());
+            sections.assign(prog->pipeW, Segments(1));
+            for (size_t i = 0; i < sops.size(); ++i) sections[pipeStageOf[i]][0].push_back(sops[i]);
+            int privBase = 0;   // private slots: liveness inside each stage, every stage in its own index range, rings behind them
+            for (auto& sec : sections) privBase += Compiler::allocateSlots(sec, ringOf, privBase);
             const int ringBase = std::max(privBase, 1);
-            nSlots = ringBase + nRing * prog->pipeDepth;
+            nSlots = ringBase + (int) ringOf.size() * prog->pipeDepth;
             if (nSlots >= MAX_SLOTS) {                                       // does not fit the 8-bit slot field: keep the program in one piece
-                piped = false; pipeStageOf.clear(); prog->pipeW = 1; prog->pipeDepth = 1;
+                sections.clear(); prog->pipeW = 1; prog->pipeDepth = 1;
             } else {
-                for (size_t i = 0; i < sops.size(); ++i) if (outSlot[i] < 0) outSlot[i] = ringBase + (-outSlot[i] - 1) * prog->pipeDepth;
+                for (auto& sec : sections)
+                    for (auto& op : sec[0]) {
+                        auto rg = ringOf.find(op.outNode);
+                        if (rg != ringOf.end()) op.slot = ringBase + rg->second * prog->pipeDepth;
+                    }
                 prog->pipeRingBase = ringBase;
             }
         }
-        if (!piped) {
-        std::unordered_map<int32_t, size_t> lastUse;
-        for (size_t i = 0; i < sops.size(); ++i)
-            if (!sops[i].isSeg) forEachSlotUse(sops[i], [&](int32_t id) { lastUse[id] = i; });
-        std::unordered_map<int32_t, int> slotOf;
-        std::vector<int> freeSlots;
-        nSlots = 0;
-        for (size_t i = 0; i < sops.size(); ++i) {
-            auto& op = sops[i];
-            if (op.isSeg) continue;
-            int s;
-            if (!freeSlots.empty()) { s = freeSlots.back(); freeSlots.pop_back(); }
-            else s = nSlots++;
-            if (s >= MAX_SLOTS) return fail(rc::InvariantViolation, "graph needs more than 255 live intermediates");
-            outSlot[i] = s;
-            slotOf[op.outNode] = s;
-            forEachSlotUse(op, [&](int32_t id) {   // free inputs whose last consumer is this op
-                auto lu = lastUse.find(id);
-                auto so = slotOf.find(id);
-                if (lu != lastUse.end() && lu->second == i && so != slotOf.end()) {
-                    freeSlots.push_back(so->second);
-                    slotOf.erase(so);
-                }
-            });
-            // an output nobody reads (root buffers, dangling nodes) is dead immediately
-            if (!lastUse.count(op.outNode)) { freeSlots.push_back(s); slotOf.erase(op.outNode); }
-        }
+        if (sections.empty()) {
+            sections.push_back(std::move(stageOps[stg]));
+            nSlots = Compiler::allocateSlots(sections[0], {}, 0);
+            if (nSlots > MAX_SLOTS) return fail(rc::InvariantViolation, "graph needs more than 255 live intermediates");
         }
         nSlotsMax = std::max(nSlotsMax, nSlots);
 
         std::unordered_map<int32_t, int> producerSlot;   // every value is produced exactly once per stage
-        for (size_t i = 0; i < sops.size(); ++i) if (!sops[i].isSeg) producerSlot[sops[i].outNode] = outSlot[i];
+        for (auto& sec : sections)
+            for (auto& ops : sec)
+                for (auto& op : ops) producerSlot[op.outNode] = op.slot;
         auto encodeOperand = [&](uint32_t kind, int32_t ref) -> uint32_t {
             if (kind == K_SLOT) {
                 auto ps = producerSlot.find(ref);
@@ -2162,28 +2080,20 @@ int Engine::compile(Group& g, int nIn, std::shared_ptr<Program>& out) {
             }
             return make_operand(K_PARAM, 0);
         };
-        auto opWords = [&](const Compiler::PendingOp& op) -> size_t {
-            if (op.isSeg) return OP_HEADER_WORDS;
+        auto operandWords = [](const PendingOp& op) -> size_t {
             size_t n = op.operands.size() + 2 * op.steps.size() + op.imm.size();
-            return OP_HEADER_WORDS + ((n + 3) & ~(size_t) 3);
+            return (n + 3) & ~(size_t) 3;
         };
-        auto emitSeg = [&](int segRoot, size_t skipWords) {
-            prog->code.push_back(make_w0(OP_SEG, 0, 0, 0));
-            prog->code.push_back(NO_STATE);
-            prog->code.push_back((uint32_t) segRoot);
-            prog->code.push_back((uint32_t) skipWords);
-            for (int k = 0; k < 4; ++k) prog->code.push_back(0);
-        };
-        auto emitOp = [&](const Compiler::PendingOp& op, int slot) -> int {
+        auto emitOp = [&](const PendingOp& op) -> int {
             ++prog->nOps;
             uint32_t st = NO_STATE;
             if (op.state != NO_STATE) {
                 auto it = g.nodes.find(op.outNode);
                 if (it != g.nodes.end()) st = mapState(it->second);
             }
-            const size_t nOperandWords = opWords(op) - OP_HEADER_WORDS;
+            const size_t nOperandWords = operandWords(op);
             if (nOperandWords > 255) return fail(rc::InvariantViolation, "operand block of one op exceeds 255 words");
-            prog->code.push_back(make_w0(op.opcode, (uint32_t) nOperandWords, (uint32_t) slot, op.mode));
+            prog->code.push_back(make_w0(op.opcode, (uint32_t) nOperandWords, (uint32_t) op.slot, op.mode));
             prog->code.push_back(st);
             prog->code.push_back(op.aux0);
             prog->code.push_back(op.opcode == OP_DELAY ? (uint32_t) ++prog->nDelayBuf : op.aux1);   // OP_DELAY: 1 + its read-window buffer
@@ -2202,35 +2112,26 @@ int Engine::compile(Group& g, int nIn, std::shared_ptr<Program>& out) {
             for (; written < nOperandWords; ++written) prog->code.push_back(0);
             return rc::Ok;
         };
-        if (piped) {
-            // one code section per pipeline stage: [SEG header][the stage's ops][END]; state rows in stage order
-            const uint32_t base = prog->stages[stg].codeOffset;
-            for (int w = 0; w < prog->pipeW; ++w) {
-                prog->pipeCode[w] = (uint32_t) prog->code.size() - base;
+        const bool piped = sections.size() > 1;
+        for (size_t w = 0; w < sections.size(); ++w) {
+            if (piped) {   // one code section per pipeline stage, closed by its own END; state rows in stage order
+                prog->pipeCode[w] = (uint32_t) prog->code.size() - prog->stages[stg].codeOffset;
                 prog->pipeState[w] = (unsigned short) prog->stateMap.size();
                 prog->pipeSrow[w] = (unsigned short) nStateRows;
-                size_t words = 0;
-                for (size_t i = 1; i < sops.size(); ++i) if (pipeStageOf[i] == w) words += opWords(sops[i]);
-                emitSeg(sops[0].segRoot, words);
-                for (size_t i = 1; i < sops.size(); ++i) {
-                    if (pipeStageOf[i] != w) continue;
-                    int r = emitOp(sops[i], outSlot[i]);
-                    if (r != rc::Ok) return r;
-                }
-                for (int k = 0; k < 8; ++k) prog->code.push_back(k == 0 ? make_w0(OP_END, 0, 0, 0) : 0u);
             }
-            for (int w = prog->pipeW; w <= MAX_PIPE; ++w) prog->pipeState[w] = (unsigned short) prog->stateMap.size();
-        } else {
-        std::vector<size_t> wordOffset(sops.size() + 1, 0);
-        for (size_t i = 0; i < sops.size(); ++i) wordOffset[i + 1] = wordOffset[i] + opWords(sops[i]);
-        for (size_t i = 0; i < sops.size(); ++i) {
-            auto& op = sops[i];
-            if (op.isSeg) { emitSeg(op.segRoot, wordOffset[op.segEndOp] - wordOffset[i + 1]); continue; }
-            int r = emitOp(op, outSlot[i]);
-            if (r != rc::Ok) return r;
+            for (size_t r = 0; r < sections[w].size(); ++r) {   // per root: [SEG header: root index, words to skip][its ops]
+                size_t words = 0;
+                for (auto& op : sections[w][r]) words += OP_HEADER_WORDS + operandWords(op);
+                prog->code.insert(prog->code.end(), {make_w0(OP_SEG, 0, 0, 0), NO_STATE, (uint32_t) r, (uint32_t) words, 0u, 0u, 0u, 0u});
+                for (auto& op : sections[w][r]) {
+                    const int rcode = emitOp(op);
+                    if (rcode != rc::Ok) return rcode;
+                }
+            }
+            if (piped) emitEnd();
         }
-        }
-        for (int k = 0; k < 8; ++k) prog->code.push_back(k == 0 ? make_w0(OP_END, 0, 0, 0) : 0u);
+        if (piped) for (int w = prog->pipeW; w <= MAX_PIPE; ++w) prog->pipeState[w] = (unsigned short) prog->stateMap.size();
+        emitEnd();
         if (stg + 1 == stageOps.size()) {   // tap promotion records live behind the last stage only
             for (auto& pr : C.promotes) {
                 Node& n = g.nodes.at(pr.second);
@@ -2243,7 +2144,7 @@ int Engine::compile(Group& g, int nIn, std::shared_ptr<Program>& out) {
                 prog->code.push_back(0); prog->code.push_back(0);
             }
         }
-        for (int k = 0; k < 8; ++k) prog->code.push_back(k == 0 ? make_w0(OP_END, 0, 0, 0) : 0u);
+        emitEnd();
     }
     prog->nStateRows = (nStateRows + 1) & ~1;
     prog->nSlots = nSlotsMax;
