@@ -644,6 +644,24 @@ __device__ __forceinline__ void render_tile(const LaunchParams& P, const int til
     // loop that stays in the instruction cache)
 #define FETCH_T(reg, j) __shfl_sync(FULL, (reg), (j) * L + vlane)
 
+#ifdef EB_SPEC_PROGRAM
+    // A specialised program with ONE root, rendering one mix-only channel: OP_ROOT (render_ops.inc) sums its faded output over the voices
+    // of the tile and stores the tile's row of the partial mix itself, so no tile clears, accumulates into and re-reads `outacc`.  The
+    // root's segment must run this block (otherwise nothing would store the row); anything else keeps the accumulate-and-epilogue path.
+    constexpr int nRoots = [] {
+        int n = 0;
+        for (int pc = 0; pc < EB_SPEC_CODE_LEN;) {
+            const uint32_t w0 = EB_SPEC_CODE[pc];
+            if ((w0 & 0xFF) == OP_END) break;
+            if ((w0 & 0xFF) == OP_ROOT) ++n;
+            pc += (int) OP_HEADER_WORDS + (int) ((w0 >> 8) & 0xFF);
+        }
+        return n;
+    }();
+    const bool rootDirect = !PIPE && nRoots == 1 && P.outVoice == nullptr && P.mixPartial != nullptr && P.nOut == 1 && (P.runMask & 1u);
+#else
+    constexpr bool rootDirect = false;
+#endif
 #ifdef EB_OPPROF
     const long long prof_tile0 = clock64();
 #endif
@@ -663,7 +681,7 @@ __device__ __forceinline__ void render_tile(const LaunchParams& P, const int til
                 __threadfence_block();
             }
         }
-        if (lastStage) for (int i = lane; i < P.nOut * E; i += 32) outacc[i] = 0.0f;
+        if (lastStage && !rootDirect) for (int i = lane; i < P.nOut * E; i += 32) outacc[i] = 0.0f;
 
 #ifdef EB_SPEC_PROGRAM
         // ---- per-program specialisation (DESIGN.md §8; compiled only when a generated header defines the program as the
@@ -671,6 +689,16 @@ __device__ __forceinline__ void render_tile(const LaunchParams& P, const int til
         // is a constant expression, so each `switch (opcode)` folds to its one case, slot addresses become immediates and chain
         // steps unroll — no dispatch, no decoding.  Device pointers (words 4/5 of a header) and the words that lanes index with
         // their own id (phasor runs, out-of-line control ops) are still read from the copy of the program in memory.
+        // Full tiles (cnt == T: every tile of a block that is a multiple of T, all but the last otherwise) run a second copy of the
+        // program in which cnt is the constant T: the `t < cnt` masks fold away, the owner-lane recurrences run exactly T steps,
+        // unrolled 8 with immediate store offsets (fully unrolled, the phasor run alone took the kernel to 128 registers), and the svf
+        // scan's identity maps for samples past cnt disappear.  A partial tile runs the same text with cnt at run time.  One warp-uniform branch per tile picks the copy; the operations and their order are the same.
+        const int tileCnt = cnt;
+        auto specTile = [&](auto fullTag) {
+        constexpr bool FULLT = decltype(fullTag)::value;
+        const int cnt = FULLT ? T : tileCnt;
+#undef FOR_OWNER
+#define FOR_OWNER(t) _Pragma("unroll (FULLT ? 8 : 4)") for (int t = 0; t < cnt; ++t)
         {
             const uint32_t* const codeMem = P.code;
             auto run = [&]<int PC, int END>(auto&& self) -> void {
@@ -718,6 +746,10 @@ __device__ __forceinline__ void render_tile(const LaunchParams& P, const int til
             };
             run.template operator()<0, EB_SPEC_CODE_LEN>(run);
         }
+#undef FOR_OWNER
+#define FOR_OWNER(t) _Pragma("unroll 4") for (int t = 0; t < cnt; ++t)
+        };
+        if (tileCnt == T) specTile(std::true_type{}); else specTile(std::false_type{});
 #else
         const uint32_t* pc = P.code + ((PIPE && pipeW > 1) ? P.pipeCode[stage] : 0u);
         for (;;) {
@@ -777,7 +809,7 @@ __device__ __forceinline__ void render_tile(const LaunchParams& P, const int til
                 }
             }
         }
-        if (P.mixPartial) {
+        if (P.mixPartial && !rootDirect) {
             // sum over the voices of the tile in a fixed order (xor butterfly over the voice bits of the lane id)
             for (int ch = 0; ch < P.nOut; ++ch) {
                 const SP a = outacc + (ch * E + lane);
@@ -878,6 +910,11 @@ constexpr int kL32MinBlocks = 8, kL1MinBlocks = 4;
 // One voice group per launch: the descriptor travels in the constant bank.
 template <int NITER, int LOGL>
 __global__ void EB_BOUNDS render_block_kernel(const __grid_constant__ LaunchParams P, const int perWarp) {
+#ifdef EB_SPEC_PROGRAM
+    // K2 is launched as this grid's programmatic dependent (launch_mix_reduce): let its CTAs take their places on the SMs this grid's
+    // early finishers leave idle.  K2 still reads the partial mix only after griddepcontrol.wait, i.e. after this whole grid.
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+#endif
     if (P.tableSmem >= 0)       // CTA-wide: one TMA bulk copy of the program's wavetable into shared memory, guarded by an mbarrier
         stage_table_tma(P.tableSrc, P.tableFloats, g_smem + P.tableSmem, reinterpret_cast<uint64_t*>(g_smem + P.tableSmem + P.tableFloats));
     const int tile = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -959,6 +996,9 @@ __global__ void __launch_bounds__(1024) mix_reduce_kernel(const float* __restric
                                                           const HostDeliver hd) {
     __shared__ float red[32][33];
     __shared__ bool last;
+    // Launched as a programmatic dependent of the K1 before it (launch_mix_reduce): wait for that grid to finish and its partial mixes
+    // to be visible.  (A no-op when the launch carries no programmatic dependency.)
+    asm volatile("griddepcontrol.wait;" ::: "memory");
     const int sx = threadIdx.x & 31, gy = threadIdx.x >> 5;       // 32 samples x 32 tile lanes
     const int chunksPerCh = (blockSize + 31) / 32;
     const int ch = blockIdx.x / chunksPerCh;
@@ -1120,8 +1160,18 @@ cudaError_t launch_mix_reduce(const float* partial, float* out, int outStride, f
     int G = (nTiles + 255) / 256;                 // ~8 tiles per lane per group; 4096 voices at L = 2 -> 8 groups x 16 chunks = 128 CTAs
     if (G > MIX_REDUCE_MAX_GROUPS) G = MIX_REDUCE_MAX_GROUPS;
     if (G < 1 || !scratch || !tickets) G = 1;
-    mix_reduce_kernel<<<dim3(nOut * chunksPerCh, G), 1024, 0, stream>>>(partial, out, scratch, tickets, nTiles, nOut, blockSize, outStride, numSamples, hd);
-    return cudaGetLastError();
+    // a programmatic dependent launch: K2's launch overlaps the tail of the K1 before it (the kernel waits for that grid on its own)
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(nOut * chunksPerCh, G);
+    cfg.blockDim = dim3(1024);
+    cfg.dynamicSmemBytes = 0;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, mix_reduce_kernel, partial, out, scratch, tickets, nTiles, nOut, blockSize, outStride, numSamples, hd);
 }
 
 // ---- K4: cross-GPU all-reduce of the mix bus over peer memory (see kernels.h) -------------------------------------------
