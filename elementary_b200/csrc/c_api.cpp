@@ -82,6 +82,12 @@ int elem_b200_set_path_per_voice(elem_b200_runtime* rt, int32_t nodeId, const ch
     GUARD(rt->engine->setPathPerVoice(nodeId, names, numNames, index, voiceBegin, count));
 }
 
+int elem_b200_reset_voices(elem_b200_runtime* rt, const int32_t* voices, size_t count) {
+    if (count > 0 && !voices) return eb::rc::BadArgument;
+    GUARD(rt->engine->resetVoices(voices, count));
+}
+uint64_t elem_b200_reset_bytes_written(elem_b200_runtime* rt) { return rt ? rt->engine->resetBytesWritten() : 0; }
+
 int elem_b200_process(elem_b200_runtime* rt, const float* const* in, size_t nIn, float* const* out, size_t nOut, size_t numSamples, void* userData) {
     GUARD(rt->engine->process(in, nIn, out, nOut, numSamples, static_cast<const int64_t*>(userData)));
 }

@@ -81,6 +81,11 @@ bool convolver_init(ConvolverState& st, IrBank& bank, const void* key, const std
 // grows (keeping every channel's most recent spectra, in order) when an IR is longer than any before.  Stream-ordered.
 bool convolver_assign(ConvolverState& st, int c0, int n, const std::vector<std::shared_ptr<IrSpectra>>& h, cudaStream_t stream, std::string& err);
 
+// What one channel owns of the state, voice-major: base + c * bytesPerChannel.  convolver_assign zeroes these regions of the channels
+// that restart; a voice reset (K6, Engine::resetVoices) zeroes them on the device.
+struct ConvRegion { void* base; size_t bytesPerChannel; };
+std::vector<ConvRegion> convolver_channel_regions(const ConvolverState& st);
+
 // Copy of channels [c0, c0+n) of `src` (same IRs, same position in the partition cycle) — used when a voice group is cut.
 bool convolver_clone_range(const ConvolverState& src, int c0, int n, ConvolverState& dst, cudaStream_t stream, std::string& err);
 // Keep only the first n channels (the other half of a cut): the unit table and descriptors are rebuilt, the storage stays.

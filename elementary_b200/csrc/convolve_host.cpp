@@ -230,14 +230,20 @@ bool convolver_assign(ConvolverState& st, int c0, int n, const std::vector<std::
     if (R > 0 && !ensureChannelBuffers(st, stream, err)) return false;
     for (int i = 0; i < n; ++i) st.chIr[(size_t) (c0 + i)] = h[(size_t) i];
     // the addressed channels restart: empty delay line, partial sums, overlap and input buffer
-    const size_t nn = (size_t) n;
-    if (st.dFdl && !zeroDev(st.dFdl + (size_t) c0 * R * CONV_PACKED_BINS, nn * R * CONV_PACKED_BINS * sizeof(float2), st.planOnly, stream, err)) return false;
-    if (st.dYpre) {
-        if (!zeroDev(st.dYpre + (size_t) c0 * CONV_PACKED_BINS, nn * CONV_PACKED_BINS * sizeof(float2), st.planOnly, stream, err)) return false;
-        if (!zeroDev(st.dOverlap + (size_t) c0 * CONV_BLOCK, nn * CONV_BLOCK * sizeof(float), st.planOnly, stream, err)) return false;
-        if (!zeroDev(st.dInBuf + (size_t) c0 * CONV_BLOCK, nn * CONV_BLOCK * sizeof(float), st.planOnly, stream, err)) return false;
-    }
+    for (const ConvRegion& r : convolver_channel_regions(st))
+        if (!zeroDev(static_cast<char*>(r.base) + (size_t) c0 * r.bytesPerChannel, (size_t) n * r.bytesPerChannel, st.planOnly, stream, err)) return false;
     return rebuildTables(st, stream, err);
+}
+
+std::vector<ConvRegion> convolver_channel_regions(const ConvolverState& st) {
+    std::vector<ConvRegion> out;
+    if (st.dFdl) out.push_back({st.dFdl, (size_t) st.partitions * CONV_PACKED_BINS * sizeof(float2)});
+    if (st.dYpre) {
+        out.push_back({st.dYpre, CONV_PACKED_BINS * sizeof(float2)});
+        out.push_back({st.dOverlap, CONV_BLOCK * sizeof(float)});
+        out.push_back({st.dInBuf, CONV_BLOCK * sizeof(float)});
+    }
+    return out;
 }
 
 bool convolver_clone_range(const ConvolverState& src, int c0, int n, ConvolverState& dst, cudaStream_t stream, std::string& err) {

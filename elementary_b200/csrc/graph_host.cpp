@@ -155,6 +155,16 @@ static const std::unordered_map<std::string, TypeInfo>& typeTable() {
     return t;
 }
 
+// Fresh state, the one definition of what a node holds right after creation: createNode writes it, compile writes a delay's again
+// when its ring is (re)allocated, and resetVoices restores it.  State row k of a node of this kind starts as freshRowBits(kind, k);
+// row shadowedRow(kind) (-1: none) is a prop the reference sets per instance (rand.seed, once.arm), restored from the node's shadow
+// row, which holds the value last set for each voice.  Rings, tap buffers and convolver state start at zero.
+static uint32_t freshRowBits(NodeKind kind, int k) {
+    if (kind == NodeKind::SparSeq && (k == 2 || k == 5 || k == 6)) return 0xFFFFFFFFu;   // SparSeq.h:353,342-345: edgeCount = -1, loopPoints = {-1, -1}
+    return 0u;                                                                          // everything else, a delay's write index included
+}
+static int shadowedRow(NodeKind kind) { return (kind == NodeKind::Rand || kind == NodeKind::Once) ? 0 : -1; }
+
 static int bitceil(int n) {   // helpers/BitUtils.h:9
     if ((n & (n - 1)) == 0) return n;
     int o = 1;
@@ -234,6 +244,8 @@ Engine::~Engine() {
     for (OfflineBuf* b : {&offOut_, &offIn_, &offMix_, &offLog_})
         for (int i = 0; i < 2; ++i) { if (b->dev[i]) cudaFree(b->dev[i]); if (b->pinned[i]) cudaFreeHost(b->pinned[i]); }
     if (dDeliverDone_) cudaFree(dDeliverDone_);
+    if (dResetPlan_) dfree(dResetPlan_);
+    if (dResetCall_) dfree(dResetCall_);
     if (wide_.dRows) dfree(wide_.dRows);
     if (wide_.dSegs) dfree(wide_.dSegs);
     if (wide_.dDst) dfree(wide_.dDst);
@@ -550,6 +562,12 @@ int Engine::createNode(Group& g, const Value& a1, const Value& a2) {   // Runtim
     if (it->second.stateRows > 0) {
         int r = allocRows(g, it->second.stateRows, it->second.evenAlign, n.stateRow);
         if (r != rc::Ok) return r;
+        for (int k = 0; k < it->second.stateRows; ++k)   // new rows are zero
+            if (freshRowBits(n.kind, k) != 0u && (r = fillRowBits(g, n.stateRow + k, 0, g.Vpad, freshRowBits(n.kind, k))) != rc::Ok) return r;
+    }
+    if (shadowedRow(n.kind) >= 0) {   // outside the state rows: no program stages it
+        int r = allocRows(g, 1, false, n.shadowRow);
+        if (r != rc::Ok) return r;
     }
     switch (n.kind) {
         case NodeKind::Const: {   // Core.h:166 default 1
@@ -565,9 +583,6 @@ int Engine::createNode(Group& g, const Value& a1, const Value& a2) {   // Runtim
         case NodeKind::Root: n.fade.init(sr_); n.channel = -1; break;          // Core.h:80-82
         case NodeKind::Delay: n.size = blockSize_; n.ringDirty = true; break;  // Delays.h:56
         case NodeKind::SDelay: n.length = blockSize_; n.size = bitceil(blockSize_ + blockSize_); n.ringDirty = true; break;   // Delays.h:183,197-198
-        case NodeKind::SparSeq: {   // SparSeq.h:353,342-345: edgeCount = -1, loopPoints = {-1, -1}
-            for (int k : {2, 5, 6}) { int r = fillRowBits(g, n.stateRow + k, 0, g.Vpad, 0xFFFFFFFFu); if (r != rc::Ok) return r; }
-        } break;
         case NodeKind::Metro: n.intervalSamps = static_cast<int64_t>(std::max(2.0, 1000.0 * 0.001 * sr_)); break;   // Metro.h:14-18
         case NodeKind::Scope:   // Analyzers.h:147-153: the constructor sets both props
             n.props["channels"] = Value::number(1); n.props["size"] = Value::number(512);
@@ -679,7 +694,9 @@ int Engine::nodeSetProperty(Group& g, Node& n, const std::string& key, const Val
         case NodeKind::Rand:        // Noise.h:13-23
             if (key == "seed") {
                 if (!val.isNumber()) return rc::InvalidPropertyType;
-                int r = fillRowBits(g, n.stateRow, vb, ve, static_cast<uint32_t>(val.asNumber()));
+                const uint32_t seed = static_cast<uint32_t>(val.asNumber());
+                int r = fillRowBits(g, n.stateRow, vb, ve, seed);
+                if (r == rc::Ok) r = fillRowBits(g, n.shadowRow, vb, ve, seed);
                 if (r != rc::Ok) return r;
             }
             break;
@@ -704,7 +721,11 @@ int Engine::nodeSetProperty(Group& g, Node& n, const std::string& key, const Val
         case NodeKind::Once:        // Core.h:345-361: the prop can arm but never disarm
             if (key == "arm") {
                 if (!val.isBool()) return rc::InvalidPropertyType;
-                if (val.asBool()) { int r = fillRow(g, n.stateRow, vb, ve, 1.0f); if (r != rc::Ok) return r; }
+                if (val.asBool()) {
+                    int r = fillRow(g, n.stateRow, vb, ve, 1.0f);
+                    if (r == rc::Ok) r = fillRow(g, n.shadowRow, vb, ve, 1.0f);
+                    if (r != rc::Ok) return r;
+                }
             }
             break;
         case NodeKind::Seq:         // Core.h:411-466
@@ -1143,16 +1164,17 @@ int Engine::setPropertyPerVoice(int32_t nodeId, const char* key, const double* v
         auto it = g.nodes.find(nodeId);
         if (it == g.nodes.end()) return rc::NodeNotFound;
         Node& n = it->second;
-        int row;
+        int row, shadow = -1;
         std::vector<uint32_t> bits((size_t) (e - b));
         if (n.kind == NodeKind::Const && k == "value") {
             row = n.paramRow;
             for (int v = b; v < e; ++v) { float f = (float) values[v - vb]; std::memcpy(&bits[v - b], &f, 4); }
         } else if (n.kind == NodeKind::Rand && k == "seed") {
-            row = n.stateRow;
+            row = n.stateRow; shadow = n.shadowRow;
             for (int v = b; v < e; ++v) bits[v - b] = static_cast<uint32_t>(values[v - vb]);
         } else return fail(rc::InvalidPropertyType, "property is not per-voice capable");
-        if (!cuda(dmemcpy(g.dRows + (size_t) row * g.Vpad + (b - g.v0), bits.data(), sizeof(uint32_t) * bits.size(), cudaMemcpyHostToDevice), "per-voice prop upload")) return rc::CudaError;   // pageable source: staged before the call returns
+        for (int r : {row, shadow})   // pageable source: staged before the call returns
+            if (r >= 0 && !cuda(dmemcpy(g.dRows + (size_t) r * g.Vpad + (b - g.v0), bits.data(), sizeof(uint32_t) * bits.size(), cudaMemcpyHostToDevice), "per-voice prop upload")) return rc::CudaError;
         n.props[k] = Value::number(values[e - 1 - vb]);
     }
     return rc::Ok;
@@ -1215,6 +1237,130 @@ int Engine::setPathPerVoice(int32_t nodeId, const char* const* names, int numNam
         n.props["path"] = Value::string(names[last]);
         if (!hadResource) g.codeDirty = true;   // the program emitted silence for a convolver without an IR
     }
+    return rc::Ok;
+}
+
+int Engine::resetVoices(const int32_t* voices, size_t count) {
+    Lock lk(mu_);
+    dsetdev();
+    if (count == 0) return rc::Ok;
+    if (!voices) return fail(rc::BadArgument, "resetVoices: null voice list");
+    std::vector<int32_t> vs(voices, voices + count);
+    for (int32_t v : vs)
+        if (v < 0 || v >= numVoices_) return fail(rc::BadArgument, "resetVoices: voice index out of range");
+    std::sort(vs.begin(), vs.end());
+    vs.erase(std::unique(vs.begin(), vs.end()), vs.end());
+
+    // runs: the voices of one voice tile; the groups they touch, in voice order
+    std::vector<int> runStart, runGroup;
+    std::vector<Group*> touched;
+    std::vector<int> touchedFirst;   // index in vs of each touched group's first voice
+    size_t gi = 0;
+    int lastTile = -1;
+    for (size_t i = 0; i < vs.size(); ++i) {
+        const int v = vs[i];
+        while (v >= groups_[gi]->v0 + groups_[gi]->nv) ++gi;
+        Group& g = *groups_[gi];
+        const int tile = (v - g.v0) / std::max(1, g.tileWidth);
+        if (touched.empty() || touched.back() != &g) { touched.push_back(&g); touchedFirst.push_back((int) i); lastTile = -1; }
+        if (tile != lastTile) { runStart.push_back((int) i); runGroup.push_back((int) touched.size() - 1); lastTile = tile; }
+    }
+    runStart.push_back((int) vs.size());
+    touchedFirst.push_back((int) vs.size());
+
+    // the reset plans of the touched groups (fresh state: freshRowBits / shadowedRow)
+    std::vector<ResetGroup> pg;
+    std::vector<ResetBuf> pb;
+    std::vector<ResetConv> pc;
+    std::vector<ResetRow> pr;
+    for (size_t t = 0; t < touched.size(); ++t) {
+        Group& g = *touched[t];
+        ResetGroup G{};
+        G.rows = g.dRows; G.v0 = g.v0; G.Vpad = g.Vpad; G.L = std::max(1, g.tileWidth);
+        G.row0 = (int) pr.size(); G.buf0 = (int) pb.size(); G.conv0 = (int) pc.size();
+        auto addBuf = [&](float* base, long long positions) {
+            if (!base || positions <= 0) return;
+            pb.push_back(ResetBuf{base, positions, G.tilePositions});
+            G.tilePositions += positions;
+        };
+        std::vector<Node*> nodes;
+        for (auto& kv : g.nodes) nodes.push_back(&kv.second);
+        std::sort(nodes.begin(), nodes.end(), [](const Node* a, const Node* b) { return a->id < b->id; });
+        for (Node* np : nodes) {
+            Node& n = *np;
+            if (n.stateRow >= 0) {
+                const bool custom = n.kind == NodeKind::Custom;
+                const int rows = custom ? customTypes_[n.fn].nState : typeTable().at(n.typeName).stateRows;
+                const bool dbl = !custom && typeTable().at(n.typeName).evenAlign;
+                for (int k = 0; k < rows; k += dbl ? 2 : 1) {
+                    if (dbl) pr.push_back(ResetRow{n.stateRow + k, RESET_ROW_DOUBLE, 0u});
+                    else if (k == shadowedRow(n.kind)) pr.push_back(ResetRow{n.stateRow + k, RESET_ROW_SHADOW, (uint32_t) n.shadowRow});
+                    else pr.push_back(ResetRow{n.stateRow + k, RESET_ROW_BITS, freshRowBits(n.kind, k)});
+                }
+            }
+            addBuf(n.ring, n.ringPositions);
+            addBuf(n.tapPrivate, blockSize_);
+            if (n.conv)
+                for (const ConvRegion& r : convolver_channel_regions(*n.conv)) {
+                    const long long quads = (long long) (r.bytesPerChannel / sizeof(float4));
+                    pc.push_back(ResetConv{static_cast<float*>(r.base), quads, G.convQuads});
+                    G.convQuads += quads;
+                }
+            for (int i = touchedFirst[t]; i < touchedFirst[t + 1] && !n.relay.empty(); ++i) {   // the host-side capture relays
+                const size_t u = (size_t) (vs[(size_t) i] - g.v0);
+                if (u < n.relay.size()) n.relay[u].clear();
+            }
+        }
+        for (auto& kv : g.tapShared) addBuf(kv.second, blockSize_);
+        G.nRows = (int) pr.size() - G.row0; G.nBufs = (int) pb.size() - G.buf0; G.nConvs = (int) pc.size() - G.conv0;
+        pg.push_back(G);
+    }
+
+    // one blob: groups, buffers, convolver regions, rows (8-byte aligned parts first); uploaded only when it changed
+    const size_t offB = pg.size() * sizeof(ResetGroup), offC = offB + pb.size() * sizeof(ResetBuf),
+                 offR = offC + pc.size() * sizeof(ResetConv), planBytes = offR + pr.size() * sizeof(ResetRow);
+    std::vector<char> blob(planBytes);
+    std::memcpy(blob.data(), pg.data(), offB);
+    if (!pb.empty()) std::memcpy(blob.data() + offB, pb.data(), offC - offB);
+    if (!pc.empty()) std::memcpy(blob.data() + offC, pc.data(), offR - offC);
+    if (!pr.empty()) std::memcpy(blob.data() + offR, pr.data(), planBytes - offR);
+    char* const oldPlan = dResetPlan_;
+    if (!grow(dResetPlan_, resetPlanCap_, planBytes, "cudaMalloc reset plan", false, 2)) return rc::CudaError;
+    if (dResetPlan_ != oldPlan || blob != resetPlanUp_) {
+        if (!cuda(dmemcpy(dResetPlan_, blob.data(), planBytes, cudaMemcpyHostToDevice), "upload reset plan")) { resetPlanUp_.clear(); return rc::CudaError; }
+        resetPlanUp_.swap(blob);
+    }
+    // the call: voices, run starts, run groups
+    const size_t nRuns = runGroup.size();
+    std::vector<int> call;
+    call.reserve(vs.size() + 2 * nRuns + 1);
+    call.insert(call.end(), vs.begin(), vs.end());
+    call.insert(call.end(), runStart.begin(), runStart.end());
+    call.insert(call.end(), runGroup.begin(), runGroup.end());
+    if (!grow(dResetCall_, resetCallCap_, call.size(), "cudaMalloc reset voices", false, 2)) return rc::CudaError;
+    if (!cuda(dmemcpy(dResetCall_, call.data(), sizeof(int) * call.size(), cudaMemcpyHostToDevice), "upload reset voices")) return rc::CudaError;   // pageable: staged before the call returns
+
+    // the slices of a run: about 2048 items per CTA for the run with the most work
+    long long maxWork = 0;
+    for (size_t r = 0; r < nRuns; ++r) {
+        const ResetGroup& G = pg[(size_t) runGroup[r]];
+        const long long m = runStart[r + 1] - runStart[r];
+        maxWork = std::max(maxWork, m * (G.nRows + G.tilePositions + G.convQuads));
+        long long bytes = m * (G.tilePositions * 4 + G.convQuads * 16);
+        for (int k = 0; k < G.nRows; ++k) bytes += m * (pr[(size_t) (G.row0 + k)].kind == RESET_ROW_DOUBLE ? 8 : 4);
+        resetBytes_ += (uint64_t) bytes;
+    }
+    const int slices = (int) std::min<long long>(65535, std::max<long long>(1, (maxWork + 2047) / 2048));
+    ResetLaunch a;
+    a.groups = reinterpret_cast<const ResetGroup*>(dResetPlan_);
+    a.bufs = reinterpret_cast<const ResetBuf*>(dResetPlan_ + offB);
+    a.convs = reinterpret_cast<const ResetConv*>(dResetPlan_ + offC);
+    a.rows = reinterpret_cast<const ResetRow*>(dResetPlan_ + offR);
+    a.voices = dResetCall_;
+    a.runStart = dResetCall_ + vs.size();
+    a.runGroup = dResetCall_ + vs.size() + nRuns + 1;
+    if (!planOnly_ && !cuda(launch_reset_voices(a, (int) nRuns, slices, stream_), "reset kernel launch")) return rc::CudaError;
+    ++launches_;
     return rc::Ok;
 }
 
@@ -1515,6 +1661,7 @@ int Compiler::emitNode(Node& n, int rootIndex) {
             if (!n.ring) {
                 if (!zeroedFloats(n.ring, floats, "analysis ring")) return rc::CudaError;
                 n.ringFloats = floats;
+                n.ringPositions = n.size;
             }
             if (n.kind == NodeKind::Scope || n.kind == NodeKind::Fft) {
                 if (numCh < 1) { zeros(); break; }
@@ -1537,8 +1684,9 @@ int Compiler::emitNode(Node& n, int rootIndex) {
                 E.dsync();
                 if (n.ring) { E.dfree(n.ring); n.ring = nullptr; }
                 n.ringFloats = (size_t) n.size * ((size_t) g.nTiles() * g.tileWidth);
+                n.ringPositions = n.size;
                 if (n.ringFloats && !zeroedFloats(n.ring, n.ringFloats, "delay ring")) return rc::CudaError;
-                int r = E.fillRowBits(g, n.stateRow, 0, g.nv, 0);   // writeIndex = 0
+                int r = E.fillRowBits(g, n.stateRow, 0, g.nv, freshRowBits(n.kind, 0));   // writeIndex
                 if (r != rc::Ok) return r;
                 n.ringDirty = false;
             }

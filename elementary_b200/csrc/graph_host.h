@@ -83,6 +83,7 @@ struct Node {
 
     int paramRow = -1;               // const / sr: per-voice parameter row
     int stateRow = -1;               // first scalar state row (even-aligned when it holds doubles)
+    int shadowRow = -1;              // rand / once: the seed / arm last set for each voice, outside the state rows (resetVoices)
     int mode = 0;                    // svf / svfshelf / mm1p mode
     int channel = 0;                 // in.channel, root.channel (-1 default for root)
     GainFade fade;                   // root
@@ -90,6 +91,7 @@ struct Node {
     bool ringDirty = true;           // (re)allocate + zero + reset writeIndex at next compile (Delays.h:92-95)
     float* ring = nullptr;
     size_t ringFloats = 0;
+    int ringPositions = 0;           // the ring is [tile][ringPositions][L] floats
     uint32_t holdSamples = 0xFFFFFFFFu;   // maxhold
     std::string tapName;
     float* tapPrivate = nullptr;     // tapOut private delayBuffer
@@ -209,6 +211,10 @@ public:
     std::vector<std::string> listSharedResources() const;
     int gc(int voice, std::vector<int32_t>& pruned);
     void reset();
+    // Voices voices[0..count) (runtime-global, any order, repeats allowed) restart as fresh instances from the next block on: state rows
+    // at their creation values (rand / once replayed from their shadow rows), their lanes of every tile buffer and their convolver
+    // regions zeroed, pending readouts and capture relays dropped.  One K6 launch, stream-ordered; no group is cut, nothing compiled.
+    int resetVoices(const int32_t* voices, size_t count);
 
     // Runtime::process shape: planar host buffers; inputs broadcast to every voice; out = mix bus.
     int process(const float* const* in, size_t nIn, float* const* out, size_t nOut, size_t numSamples, const int64_t* sampleTime = nullptr);
@@ -261,6 +267,7 @@ public:
     int numVoices() const { return numVoices_; }
     int blockSize() const { return blockSize_; }
     uint64_t kernelLaunches() const { Lock lk(mu_); return launches_; }
+    uint64_t resetBytesWritten() const { Lock lk(mu_); return resetBytes_; }
     // The int64 sample clock handed to nodes through BlockContext::userData (wasm/Main.cpp:206-217, Metro.h:44,
     // SampleTime.h:19).  process() takes it from *userData when given; otherwise the engine counts samples itself.
     // Runtime::processQueuedEvents (Runtime.h:64,438-446): events of the voices [vb, ve); cb(type, event JSON, voice).
@@ -431,6 +438,12 @@ private:
     int launchWide(const BlockIO& io);
     // the mix channels of a program: distinct channels in [0, nOut) of all its roots, running or fading, ascending
     std::vector<int> mixChannels(const Group& g, const Program& p, size_t nOut) const;
+
+    // K6 (resetVoices): the reset plans of the groups a call touches, as last uploaded, and the call's voice list and runs
+    std::vector<char> resetPlanUp_;
+    char* dResetPlan_ = nullptr; size_t resetPlanCap_ = 0;
+    int* dResetCall_ = nullptr; size_t resetCallCap_ = 0;
+    uint64_t resetBytes_ = 0;            // bytes the reset launches wrote so far (from the plans)
 
     // K4 state
     void* dExchange_ = nullptr; size_t exchangeBytes_ = 0; size_t exchangeFlagOffset_ = 0, exchangeOwnOffset_ = 0;

@@ -96,6 +96,25 @@ constexpr int EVENT_LOG_BATCH = 32;   // items per launch (the batch travels as 
 struct EventLogBatch { int n; EventLogItem item[EVENT_LOG_BATCH]; };
 cudaError_t launch_event_log(const EventLogBatch& batch, cudaStream_t stream);
 
+// K6 (reset_kernel.cu): voices restart as fresh instances (Engine::resetVoices).  The reset plan of a voice group lists what a voice
+// owns: cells of state rows, lanes of tile-structured buffers [tile][pos][L] and voice-major convolver regions.  One launch covers the
+// runs of a call — the sorted voices of one voice tile each, voices[runStart[r] .. runStart[r + 1]) in group runGroup[r].
+enum ResetRowKind : uint32_t { RESET_ROW_BITS = 0, RESET_ROW_DOUBLE = 1, RESET_ROW_SHADOW = 2 };
+struct ResetRow { int row; uint32_t kind; uint32_t value; };   // BITS: the creation bits; DOUBLE: a double pair row, zeroed; SHADOW: value = shadow row
+struct ResetBuf { float* base; long long positions, pos0; };  // [tile][positions][L] floats; pos0: positions of the group's earlier buffers
+struct ResetConv { float* base; long long quads, quad0; };    // [voice][quads] float4; quad0: quads of the group's earlier regions
+struct ResetGroup {
+    float* rows;
+    int v0, Vpad, L;
+    int row0, nRows, buf0, nBufs, conv0, nConvs;              // the group's entries of the plan arrays
+    long long tilePositions, convQuads;                       // sums over its buffers / regions
+};
+struct ResetLaunch {
+    const ResetGroup* groups; const ResetRow* rows; const ResetBuf* bufs; const ResetConv* convs;
+    const int* voices; const int* runStart; const int* runGroup;
+};
+cudaError_t launch_reset_voices(const ResetLaunch& a, int nRuns, int slices, cudaStream_t stream);
+
 // A/B builds (-DEB_OPPROF): cycles / dispatches per opcode of the interpreter; zeros in the product library.
 cudaError_t debug_opprof_read(unsigned long long* out128, bool reset);
 

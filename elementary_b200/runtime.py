@@ -63,6 +63,10 @@ def load_library() -> C.CDLL:
     lib.elem_b200_set_property_per_voice.argtypes = [C.c_void_p, C.c_int32, C.c_char_p, C.POINTER(C.c_double), C.c_int, C.c_int]
     lib.elem_b200_set_path_per_voice.restype = C.c_int
     lib.elem_b200_set_path_per_voice.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), C.c_int, C.POINTER(C.c_int32), C.c_int, C.c_int]
+    lib.elem_b200_reset_voices.restype = C.c_int
+    lib.elem_b200_reset_voices.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_size_t]
+    lib.elem_b200_reset_bytes_written.restype = C.c_uint64
+    lib.elem_b200_reset_bytes_written.argtypes = [C.c_void_p]
     lib.elem_b200_process.restype = C.c_int
     lib.elem_b200_process.argtypes = [C.c_void_p, _f32pp, C.c_size_t, _f32pp, C.c_size_t, C.c_size_t, C.c_void_p]
     lib.elem_b200_set_current_time.argtypes = [C.c_void_p, C.c_int64]
@@ -219,6 +223,21 @@ class Runtime:
         idx = np.ascontiguousarray(np.asarray(index, dtype=np.int32).reshape(-1))
         return self._lib.elem_b200_set_path_per_voice(self._h, int(node_id), tab, len(enc),
                                                       idx.ctypes.data_as(C.POINTER(C.c_int32)), int(voice_begin), idx.size)
+
+    def reset_voices(self, voices) -> int:
+        """The given voices (runtime-global indices, any order, repeats allowed) restart as fresh instances from the next block on, as
+        if a new Runtime had been given this runtime's instruction history; props are replayed as last set for each voice.  One kernel
+        launch, stream-ordered, no voice group cut.  Returns 0, or -2 (nothing changed) when an index is outside [0, num_voices)."""
+        v = np.ascontiguousarray(np.asarray(voices, dtype=np.int64).reshape(-1))
+        if v.size and (v.min() < -2**31 or v.max() >= 2**31):
+            return -2
+        v = v.astype(np.int32)
+        return self._lib.elem_b200_reset_voices(self._h, v.ctypes.data_as(C.POINTER(C.c_int32)), v.size)
+
+    @property
+    def reset_bytes_written(self) -> int:
+        """Bytes the voice resets have written so far, counted from their plans."""
+        return int(self._lib.elem_b200_reset_bytes_written(self._h))
 
     # -- Runtime::process (Runtime.h:51-57,275-290): out = mix bus over all voices -------------------------------
     def process(self, inputs: Optional[np.ndarray], num_outputs: int, num_samples: Optional[int] = None,

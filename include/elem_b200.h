@@ -79,6 +79,21 @@ int elem_b200_set_property_per_voice(elem_b200_runtime* rt, int32_t nodeId, cons
 int elem_b200_set_path_per_voice(elem_b200_runtime* rt, int32_t nodeId, const char* const* names, int numNames,
                                  const int32_t* index, int voiceBegin, int count);
 
+/* Voices voices[0..count) restart as fresh instances: each renders from its next block on what a Runtime newly
+ * created and given this runtime's instruction history would render. Props are replayed as last set for that voice.
+ * Stream-ordered: applied between the previous and the next block, with no host synchronisation. No voice group is
+ * cut, nothing is recompiled, and snapshot() and the groups and programs in describe() do not change.
+ * Indices are runtime-global and may be unsorted or repeated; one outside [0, numVoices) returns -2 and nothing changes;
+ * count == 0 launches nothing.  Call it from the control thread, like elem_b200_set_property_per_voice.
+ * Shared by a voice group, so not restarted: root fades, the scope / fft window positions, the metro flag, the sample clock and
+ * the convolver's partition phase — a reset voice's convolver is a fresh one fed zeros since the last 512-sample partition
+ * boundary, as after elem_b200_set_path_per_voice.  No reference method: the equivalent of constructing a new Runtime for
+ * that voice. */
+int elem_b200_reset_voices(elem_b200_runtime* rt, const int32_t* voices, size_t count);
+/* Bytes the voice resets of this runtime have written so far, counted from their plans (state cells, buffer lanes, convolver
+ * regions). */
+uint64_t elem_b200_reset_bytes_written(elem_b200_runtime* rt);
+
 /* Runtime::process(in, nIn, out, nOut, numSamples, userData) — Runtime.h:51-57,275-290.
  * `in` channels are broadcast to every voice; out[c] receives the MIX BUS: the sum over all voices of what
  * each voice's Runtime would have written to its out[c].  Host buffers; the H2D copy of the inputs and the hand-over of the
