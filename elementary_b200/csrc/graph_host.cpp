@@ -104,53 +104,54 @@ Program::~Program() {
 
 DeviceArray::~DeviceArray() { if (d) rawFree(d, planOnly); }
 
-struct TypeInfo { NodeKind kind; uint32_t fn; int stateRows; bool evenAlign; };
+struct TypeInfo { NodeKind kind; uint32_t fn; int stateRows; int doubleRows; };   // doubleRows: the leading state rows that are double pairs
 
 // Registered builtin names: DefaultNodeTypes.h:53-143 (+ "convolve", "metro", "time": wasm/Main.cpp:47-61).  Types that
-// are out of scope (SURVEY.md §2d: sample*, mc.*) are deliberately absent and yield UnknownNodeType like any
+// are out of scope (SURVEY.md §2d: sampleseq, sampleseq2, mc.*) are deliberately absent and yield UnknownNodeType like any
 // unregistered name (Runtime.h:304-305).
 static const std::unordered_map<std::string, TypeInfo>& typeTable() {
     static const std::unordered_map<std::string, TypeInfo> t = {
-        {"in", {NodeKind::In, 0, 0, false}},
-        {"sin", {NodeKind::Unary, F_SIN, 0, false}}, {"cos", {NodeKind::Unary, F_COS, 0, false}},
-        {"tan", {NodeKind::Unary, F_TAN, 0, false}}, {"tanh", {NodeKind::Unary, F_TANH, 0, false}},
-        {"asinh", {NodeKind::Unary, F_ASINH, 0, false}}, {"ln", {NodeKind::Unary, F_LN, 0, false}},
-        {"log", {NodeKind::Unary, F_LOG10, 0, false}}, {"log2", {NodeKind::Unary, F_LOG2, 0, false}},
-        {"ceil", {NodeKind::Unary, F_CEIL, 0, false}}, {"floor", {NodeKind::Unary, F_FLOOR, 0, false}},
-        {"round", {NodeKind::Unary, F_ROUND, 0, false}}, {"sqrt", {NodeKind::Unary, F_SQRT, 0, false}},
-        {"exp", {NodeKind::Unary, F_EXP, 0, false}}, {"abs", {NodeKind::Unary, F_ABS, 0, false}},
-        {"le", {NodeKind::Binary, F_LE, 0, false}}, {"leq", {NodeKind::Binary, F_LEQ, 0, false}},
-        {"ge", {NodeKind::Binary, F_GE, 0, false}}, {"geq", {NodeKind::Binary, F_GEQ, 0, false}},
-        {"pow", {NodeKind::Binary, F_POW, 0, false}}, {"eq", {NodeKind::Binary, F_EQ, 0, false}},
-        {"and", {NodeKind::Binary, F_AND, 0, false}}, {"or", {NodeKind::Binary, F_OR, 0, false}},
-        {"add", {NodeKind::Reduce, F_ADD, 0, false}}, {"sub", {NodeKind::Reduce, F_SUB, 0, false}},
-        {"mul", {NodeKind::Reduce, F_MUL, 0, false}}, {"div", {NodeKind::Reduce, F_DIV, 0, false}},
-        {"mod", {NodeKind::Reduce, F_MOD, 0, false}}, {"min", {NodeKind::Reduce, F_MIN, 0, false}},
-        {"max", {NodeKind::Reduce, F_MAX, 0, false}},
-        {"root", {NodeKind::Root, 0, 0, false}}, {"const", {NodeKind::Const, 0, 0, false}},
-        {"sr", {NodeKind::Sr, 0, 0, false}},
-        {"phasor", {NodeKind::Phasor, 0, 1, false}}, {"sphasor", {NodeKind::SPhasor, 0, 2, false}},
-        {"counter", {NodeKind::Counter, 0, 1, false}}, {"accum", {NodeKind::Accum, 0, 2, false}},
-        {"latch", {NodeKind::Latch, 0, 2, false}}, {"maxhold", {NodeKind::MaxHold, 0, 3, false}},
-        {"rand", {NodeKind::Rand, 0, 1, false}},
-        {"delay", {NodeKind::Delay, 0, 1, false}}, {"sdelay", {NodeKind::SDelay, 0, 1, false}},
-        {"z", {NodeKind::Z, 0, 1, false}},
-        {"pole", {NodeKind::Pole, 0, 1, false}}, {"env", {NodeKind::Env, 0, 1, false}},
-        {"biquad", {NodeKind::Biquad, 0, 2, false}}, {"prewarp", {NodeKind::Prewarp, 0, 0, false}},
-        {"mm1p", {NodeKind::MM1p, 0, 2, true}}, {"svf", {NodeKind::Svf, 0, 4, true}},
-        {"svfshelf", {NodeKind::SvfShelf, 0, 4, true}},
-        {"tapIn", {NodeKind::TapIn, 0, 0, false}}, {"tapOut", {NodeKind::TapOut, 0, 0, false}},
-        {"table", {NodeKind::Table, 0, 0, false}},
-        {"blepsaw", {NodeKind::Blep, 0, 2, false}}, {"blepsquare", {NodeKind::Blep, 1, 2, false}},
-        {"bleptriangle", {NodeKind::Blep, 2, 2, false}},
-        {"convolve", {NodeKind::Convolve, 0, 0, false}},
-        {"once", {NodeKind::Once, 0, 4, false}}, {"seq", {NodeKind::Seq, 0, 6, false}},
-        {"seq2", {NodeKind::Seq2, 0, 3, false}}, {"sparseq", {NodeKind::SparSeq, 0, 13, false}},
-        {"sparseq2", {NodeKind::SparSeq2, 0, 3, false}},
-        {"time", {NodeKind::Time, 0, 0, false}}, {"metro", {NodeKind::Metro, 0, 0, false}},
-        {"meter", {NodeKind::Meter, 0, 3, false}}, {"snapshot", {NodeKind::Snapshot, 0, 3, false}},
-        {"scope", {NodeKind::Scope, 0, 0, false}}, {"capture", {NodeKind::Capture, 0, 5, false}},
-        {"fft", {NodeKind::Fft, 0, 0, false}},
+        {"in", {NodeKind::In, 0, 0, 0}},
+        {"sin", {NodeKind::Unary, F_SIN, 0, 0}}, {"cos", {NodeKind::Unary, F_COS, 0, 0}},
+        {"tan", {NodeKind::Unary, F_TAN, 0, 0}}, {"tanh", {NodeKind::Unary, F_TANH, 0, 0}},
+        {"asinh", {NodeKind::Unary, F_ASINH, 0, 0}}, {"ln", {NodeKind::Unary, F_LN, 0, 0}},
+        {"log", {NodeKind::Unary, F_LOG10, 0, 0}}, {"log2", {NodeKind::Unary, F_LOG2, 0, 0}},
+        {"ceil", {NodeKind::Unary, F_CEIL, 0, 0}}, {"floor", {NodeKind::Unary, F_FLOOR, 0, 0}},
+        {"round", {NodeKind::Unary, F_ROUND, 0, 0}}, {"sqrt", {NodeKind::Unary, F_SQRT, 0, 0}},
+        {"exp", {NodeKind::Unary, F_EXP, 0, 0}}, {"abs", {NodeKind::Unary, F_ABS, 0, 0}},
+        {"le", {NodeKind::Binary, F_LE, 0, 0}}, {"leq", {NodeKind::Binary, F_LEQ, 0, 0}},
+        {"ge", {NodeKind::Binary, F_GE, 0, 0}}, {"geq", {NodeKind::Binary, F_GEQ, 0, 0}},
+        {"pow", {NodeKind::Binary, F_POW, 0, 0}}, {"eq", {NodeKind::Binary, F_EQ, 0, 0}},
+        {"and", {NodeKind::Binary, F_AND, 0, 0}}, {"or", {NodeKind::Binary, F_OR, 0, 0}},
+        {"add", {NodeKind::Reduce, F_ADD, 0, 0}}, {"sub", {NodeKind::Reduce, F_SUB, 0, 0}},
+        {"mul", {NodeKind::Reduce, F_MUL, 0, 0}}, {"div", {NodeKind::Reduce, F_DIV, 0, 0}},
+        {"mod", {NodeKind::Reduce, F_MOD, 0, 0}}, {"min", {NodeKind::Reduce, F_MIN, 0, 0}},
+        {"max", {NodeKind::Reduce, F_MAX, 0, 0}},
+        {"root", {NodeKind::Root, 0, 0, 0}}, {"const", {NodeKind::Const, 0, 0, 0}},
+        {"sr", {NodeKind::Sr, 0, 0, 0}},
+        {"phasor", {NodeKind::Phasor, 0, 1, 0}}, {"sphasor", {NodeKind::SPhasor, 0, 2, 0}},
+        {"counter", {NodeKind::Counter, 0, 1, 0}}, {"accum", {NodeKind::Accum, 0, 2, 0}},
+        {"latch", {NodeKind::Latch, 0, 2, 0}}, {"maxhold", {NodeKind::MaxHold, 0, 3, 0}},
+        {"rand", {NodeKind::Rand, 0, 1, 0}},
+        {"delay", {NodeKind::Delay, 0, 1, 0}}, {"sdelay", {NodeKind::SDelay, 0, 1, 0}},
+        {"z", {NodeKind::Z, 0, 1, 0}},
+        {"pole", {NodeKind::Pole, 0, 1, 0}}, {"env", {NodeKind::Env, 0, 1, 0}},
+        {"biquad", {NodeKind::Biquad, 0, 2, 0}}, {"prewarp", {NodeKind::Prewarp, 0, 0, 0}},
+        {"mm1p", {NodeKind::MM1p, 0, 2, 2}}, {"svf", {NodeKind::Svf, 0, 4, 4}},
+        {"svfshelf", {NodeKind::SvfShelf, 0, 4, 4}},
+        {"tapIn", {NodeKind::TapIn, 0, 0, 0}}, {"tapOut", {NodeKind::TapOut, 0, 0, 0}},
+        {"table", {NodeKind::Table, 0, 0, 0}},
+        {"blepsaw", {NodeKind::Blep, 0, 2, 0}}, {"blepsquare", {NodeKind::Blep, 1, 2, 0}},
+        {"bleptriangle", {NodeKind::Blep, 2, 2, 0}},
+        {"convolve", {NodeKind::Convolve, 0, 0, 0}},
+        {"once", {NodeKind::Once, 0, 4, 0}}, {"seq", {NodeKind::Seq, 0, 6, 0}},
+        {"seq2", {NodeKind::Seq2, 0, 3, 0}}, {"sparseq", {NodeKind::SparSeq, 0, 13, 0}},
+        {"sparseq2", {NodeKind::SparSeq2, 0, 3, 0}},
+        {"time", {NodeKind::Time, 0, 0, 0}}, {"metro", {NodeKind::Metro, 0, 0, 0}},
+        {"meter", {NodeKind::Meter, 0, 3, 0}}, {"snapshot", {NodeKind::Snapshot, 0, 3, 0}},
+        {"scope", {NodeKind::Scope, 0, 0, 0}}, {"capture", {NodeKind::Capture, 0, 5, 0}},
+        {"fft", {NodeKind::Fft, 0, 0, 0}},
+        {"sample", {NodeKind::Sample, 0, 10, 4}},   // two reader positions (double), gains, change.lastIn, currentReader
     };
     return t;
 }
@@ -560,7 +561,7 @@ int Engine::createNode(Group& g, const Value& a1, const Value& a2) {   // Runtim
     n.fn = it->second.fn;
     n.typeName = a2.asString();
     if (it->second.stateRows > 0) {
-        int r = allocRows(g, it->second.stateRows, it->second.evenAlign, n.stateRow);
+        int r = allocRows(g, it->second.stateRows, it->second.doubleRows > 0, n.stateRow);
         if (r != rc::Ok) return r;
         for (int k = 0; k < it->second.stateRows; ++k)   // new rows are zero
             if (freshRowBits(n.kind, k) != 0u && (r = fillRowBits(g, n.stateRow + k, 0, g.Vpad, freshRowBits(n.kind, k))) != rc::Ok) return r;
@@ -588,6 +589,11 @@ int Engine::createNode(Group& g, const Value& a1, const Value& a2) {   // Runtim
             n.props["channels"] = Value::number(1); n.props["size"] = Value::number(512);
             n.size = SCOPE_CHANNELS * SCOPE_RING; break;
         case NodeKind::Capture: n.size = bitceil((int) (size_t) sr_) + CAPTURE_SCRATCH; break;   // Capture.h:17
+        case NodeKind::Sample: {   // buffer pointer lo / hi, length + 1 (0: no buffer), startOffset, stopOffset: new rows are zero
+            int r = allocRows(g, 5, false, n.paramRow);
+            if (r != rc::Ok) return r;
+            n.voiceRes.assign((size_t) g.nv, nullptr);
+        } break;
         case NodeKind::Fft: {   // wasm/FFT.h:18-26: ring of one channel, default size 1024 set through setProperty
             n.size = SCOPE_RING;
             Node& ref = g.nodes.emplace(id, std::move(n)).first->second;
@@ -715,6 +721,30 @@ int Engine::nodeSetProperty(Group& g, Node& n, const std::string& key, const Val
                 if (it == resources_.end()) return rc::InvalidPropertyValue;
                 n.resource = it->second;
                 n.resourceDirty = true; g.codeDirty = true;
+            }
+            break;
+        case NodeKind::Sample:      // Sample.h:25-76
+            if (key == "path") {
+                if (!val.isString()) return rc::InvalidPropertyType;
+                auto it = resources_.find(val.asString());
+                if (it == resources_.end()) return rc::InvalidPropertyValue;
+                std::vector<std::shared_ptr<Resource>> res(1, it->second);
+                std::vector<int32_t> index((size_t) (ve - vb), 0);
+                int r = assignSampleBuffers(g, n, res, index.data(), vb, ve);
+                if (r != rc::Ok) return r;
+            }
+            if (key == "mode") {
+                if (!val.isString()) return rc::InvalidPropertyType;
+                const std::string& m = val.asString();
+                if (m == "trigger") n.mode = 0; if (m == "gate") n.mode = 1; if (m == "loop") n.mode = 2;
+                g.codeDirty = true;
+            }
+            if (key == "startOffset" || key == "stopOffset") {
+                if (!val.isNumber()) return rc::InvalidPropertyType;
+                const int v = static_cast<int>(val.asNumber());
+                if (v < 0) return rc::InvalidPropertyValue;
+                int r = fillRowBits(g, n.paramRow + (key == "startOffset" ? 3 : 4), vb, ve, (uint32_t) v);
+                if (r != rc::Ok) return r;
             }
             break;
 
@@ -920,7 +950,7 @@ int Engine::applyToGroup(Group& g, const std::vector<Value>& batch, int vb, int 
 }
 
 bool Engine::isValueOnlyBatch(const std::vector<Value>& batch, int vb, int ve) {
-    // A batch made only of SET_PROPERTY on per-voice-capable props (const.value, rand.seed, once.arm) never changes the
+    // A batch made only of SET_PROPERTY on per-voice-capable props (const.value, rand.seed, once.arm, sample.startOffset / stopOffset) never changes the
     // structure of a group, so it may address any sub-range of voices without splitting the group.
     for (auto& ins : batch) {
         if (!ins.isArray()) return false;
@@ -934,7 +964,8 @@ bool Engine::isValueOnlyBatch(const std::vector<Value>& batch, int vb, int ve) {
             if (it == g->nodes.end()) return false;
             const bool ok = (it->second.kind == NodeKind::Const && ar[2].asString() == "value" && ar[3].isNumber()) ||
                             (it->second.kind == NodeKind::Rand && ar[2].asString() == "seed" && ar[3].isNumber()) ||
-                            (it->second.kind == NodeKind::Once && ar[2].asString() == "arm" && ar[3].isBool());
+                            (it->second.kind == NodeKind::Once && ar[2].asString() == "arm" && ar[3].isBool()) ||
+                            (it->second.kind == NodeKind::Sample && (ar[2].asString() == "startOffset" || ar[2].asString() == "stopOffset") && ar[3].isNumber());
             if (!ok) return false;
         }
     }
@@ -973,7 +1004,7 @@ int Engine::splitGroupsAt(int v) {
                 const Node& n = kv.second;
                 if (n.kind == NodeKind::Custom) continue;     // registered types keep float state only
                 const auto& ti = typeTable().at(n.typeName);
-                if (ti.evenAlign && n.stateRow >= 0) for (int k = 0; k < ti.stateRows; k += 2) isDoublePair[(size_t) n.stateRow + k] = 1;
+                if (n.stateRow >= 0) for (int k = 0; k < ti.doubleRows; k += 2) isDoublePair[(size_t) n.stateRow + k] = 1;
             }
             for (int r = 0; r < g.rowsUsed; ++r) {
                 if (isDoublePair[(size_t) r]) {
@@ -1006,6 +1037,10 @@ int Engine::splitGroupsAt(int v) {
             if (!kv.second.relay.empty()) {   // capture relay buffers follow their voices
                 n.relay.assign(kv.second.relay.begin() + std::min<size_t>(cut, kv.second.relay.size()), kv.second.relay.end());
                 kv.second.relay.resize(std::min<size_t>(cut, kv.second.relay.size()));
+            }
+            if (!kv.second.voiceRes.empty()) {   // so do the buffers sample voices play
+                n.voiceRes.assign(kv.second.voiceRes.begin() + std::min<size_t>(cut, kv.second.voiceRes.size()), kv.second.voiceRes.end());
+                kv.second.voiceRes.resize(std::min<size_t>(cut, kv.second.voiceRes.size()));
             }
             if (kv.second.ring) {
                 if (!cloneTiles(kv.second.ring, (size_t) kv.second.size * L, &n.ring)) return rc::CudaError;
@@ -1157,13 +1192,25 @@ int Engine::setPropertyPerVoice(int32_t nodeId, const char* key, const double* v
     dsetdev();
     if (vb < 0 || count < 0 || vb + count > numVoices_) return fail(rc::BadArgument, "voice range out of bounds");
     const std::string k(key);
+    const bool offsetKey = k == "startOffset" || k == "stopOffset";
+    // every check before any change: a failed call changes nothing
+    for (auto& gp : groups_) {
+        const Group& g = *gp;
+        if (std::max(vb, g.v0) >= std::min(vb + count, g.v0 + g.nv)) continue;
+        auto it = g.nodes.find(nodeId);
+        if (it == g.nodes.end()) return rc::NodeNotFound;
+        const NodeKind kind = it->second.kind;
+        if (!((kind == NodeKind::Const && k == "value") || (kind == NodeKind::Rand && k == "seed") || (kind == NodeKind::Sample && offsetKey)))
+            return fail(rc::InvalidPropertyType, "property is not per-voice capable");
+    }
+    if (offsetKey)
+        for (int i = 0; i < count; ++i)
+            if (static_cast<int>(values[i]) < 0) return fail(rc::InvalidPropertyValue, "sample offsets must not be negative");   // Sample.h:56,69
     for (auto& gp : groups_) {
         Group& g = *gp;
         const int b = std::max(vb, g.v0), e = std::min(vb + count, g.v0 + g.nv);
         if (b >= e) continue;
-        auto it = g.nodes.find(nodeId);
-        if (it == g.nodes.end()) return rc::NodeNotFound;
-        Node& n = it->second;
+        Node& n = g.nodes.find(nodeId)->second;
         int row, shadow = -1;
         std::vector<uint32_t> bits((size_t) (e - b));
         if (n.kind == NodeKind::Const && k == "value") {
@@ -1172,7 +1219,10 @@ int Engine::setPropertyPerVoice(int32_t nodeId, const char* key, const double* v
         } else if (n.kind == NodeKind::Rand && k == "seed") {
             row = n.stateRow; shadow = n.shadowRow;
             for (int v = b; v < e; ++v) bits[v - b] = static_cast<uint32_t>(values[v - vb]);
-        } else return fail(rc::InvalidPropertyType, "property is not per-voice capable");
+        } else {   // sample startOffset / stopOffset
+            row = n.paramRow + (k == "startOffset" ? 3 : 4);
+            for (int v = b; v < e; ++v) bits[v - b] = (uint32_t) static_cast<int>(values[v - vb]);
+        }
         for (int r : {row, shadow})   // pageable source: staged before the call returns
             if (r >= 0 && !cuda(dmemcpy(g.dRows + (size_t) r * g.Vpad + (b - g.v0), bits.data(), sizeof(uint32_t) * bits.size(), cudaMemcpyHostToDevice), "per-voice prop upload")) return rc::CudaError;
         n.props[k] = Value::number(values[e - 1 - vb]);
@@ -1192,7 +1242,7 @@ int Engine::setPathPerVoice(int32_t nodeId, const char* const* names, int numNam
         if (std::max(vb, g.v0) >= std::min(vb + count, g.v0 + g.nv)) continue;
         auto it = g.nodes.find(nodeId);
         if (it == g.nodes.end()) return rc::NodeNotFound;
-        if (it->second.kind != NodeKind::Convolve) return fail(rc::InvalidPropertyType, "property is not per-voice capable");
+        if (it->second.kind != NodeKind::Convolve && it->second.kind != NodeKind::Sample) return fail(rc::InvalidPropertyType, "property is not per-voice capable");
     }
     std::vector<std::shared_ptr<Resource>> res((size_t) numNames);
     for (int k = 0; k < numNames; ++k) {
@@ -1217,6 +1267,12 @@ int Engine::setPathPerVoice(int32_t nodeId, const char* const* names, int numNam
         const int b = std::max(vb, g.v0), e = std::min(vb + count, g.v0 + g.nv);
         if (b >= e) continue;
         Node& n = g.nodes.find(nodeId)->second;
+        if (n.kind == NodeKind::Sample) {
+            const int r = assignSampleBuffers(g, n, res, index + (b - vb), b - g.v0, e - g.v0);
+            if (r != rc::Ok) return r;
+            n.props["path"] = Value::string(names[index[e - 1 - vb]]);
+            continue;
+        }
         std::string err;
         const bool hadResource = (bool) n.resource;
         if (n.resourceDirty || !n.conv) {
@@ -1291,11 +1347,13 @@ int Engine::resetVoices(const int32_t* voices, size_t count) {
             if (n.stateRow >= 0) {
                 const bool custom = n.kind == NodeKind::Custom;
                 const int rows = custom ? customTypes_[n.fn].nState : typeTable().at(n.typeName).stateRows;
-                const bool dbl = !custom && typeTable().at(n.typeName).evenAlign;
-                for (int k = 0; k < rows; k += dbl ? 2 : 1) {
+                const int dblRows = custom ? 0 : typeTable().at(n.typeName).doubleRows;
+                for (int k = 0; k < rows;) {
+                    const bool dbl = k < dblRows;
                     if (dbl) pr.push_back(ResetRow{n.stateRow + k, RESET_ROW_DOUBLE, 0u});
                     else if (k == shadowedRow(n.kind)) pr.push_back(ResetRow{n.stateRow + k, RESET_ROW_SHADOW, (uint32_t) n.shadowRow});
                     else pr.push_back(ResetRow{n.stateRow + k, RESET_ROW_BITS, freshRowBits(n.kind, k)});
+                    k += dbl ? 2 : 1;
                 }
             }
             addBuf(n.ring, n.ringPositions);
@@ -1390,7 +1448,38 @@ int Engine::gc(int voice, std::vector<int32_t>& pruned) {
 
 void Engine::reset() {
     Lock lk(mu_);
-    // Runtime.h:449-458: only SampleNode does anything on reset() in the reference; no in-scope node does.
+    // Runtime.h:449-458: only SampleNode does anything on reset(): noteOff on both readers (targetGain rows 4 and 6)
+    dsetdev();
+    for (auto& gp : groups_)
+        for (auto& kv : gp->nodes)
+            if (kv.second.kind == NodeKind::Sample)
+                for (int k : {4, 6}) fillRowBits(*gp, kv.second.stateRow + k, 0, gp->nv, 0u);
+}
+
+// Voice vb + i (group-relative, i < ve - vb) of sample node n plays res[index[i]] from the next block on with fresh readers
+// (Sample.h:94-99: gain 0, target 0, pos 0); currentReader and change.lastIn are kept.
+int Engine::assignSampleBuffers(Group& g, Node& n, const std::vector<std::shared_ptr<Resource>>& res, const int32_t* index, int vb, int ve) {
+    const int cnt = ve - vb;
+    if (cnt <= 0) return rc::Ok;
+    for (auto& r : res) { const int e = ensureResourceOnDevice(*r); if (e != rc::Ok) return e; }
+    std::vector<uint32_t> desc((size_t) 3 * cnt);
+    for (int i = 0; i < cnt; ++i) {
+        const Resource& r = *res[(size_t) index[i]];
+        const uint64_t p = (uint64_t) (uintptr_t) r.dChannel0;
+        desc[(size_t) i] = (uint32_t) p;
+        desc[(size_t) cnt + i] = (uint32_t) (p >> 32);
+        desc[(size_t) 2 * cnt + i] = (uint32_t) r.numSamples + 1u;
+    }
+    for (int k = 0; k < 3; ++k)   // pageable source: staged before the call returns
+        if (!cuda(dmemcpy(g.dRows + (size_t) (n.paramRow + k) * g.Vpad + vb, desc.data() + (size_t) k * cnt, sizeof(uint32_t) * cnt, cudaMemcpyHostToDevice), "sample buffer rows")) return rc::CudaError;
+    // reader state: two double rows (the positions, 2 * vb ..) then the four gain rows
+    if (!cuda(dmemset(g.dRows + (size_t) n.stateRow * g.Vpad + 2 * (size_t) vb, 0, sizeof(double) * cnt), "sample reader reset")) return rc::CudaError;
+    if (!cuda(dmemset(g.dRows + (size_t) (n.stateRow + 2) * g.Vpad + 2 * (size_t) vb, 0, sizeof(double) * cnt), "sample reader reset")) return rc::CudaError;
+    for (int k = 4; k < 8; ++k) { const int e = fillRowBits(g, n.stateRow + k, vb, ve, 0u); if (e != rc::Ok) return e; }
+    if (n.voiceRes.size() < (size_t) g.nv) n.voiceRes.resize((size_t) g.nv);
+    for (int i = 0; i < cnt; ++i) n.voiceRes[(size_t) (vb + i)] = res[(size_t) index[i]];
+    steadyValid_ = false;
+    return rc::Ok;
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -1708,6 +1797,15 @@ int Compiler::emitNode(Node& n, int rootIndex) {
                 prog.stagedTable = n.resource->dChannel0;
                 prog.stagedTableFloats = (int) ((n.resource->numSamples + 3) / 4 * 4);
             }
+        } break;
+
+        case NodeKind::Sample: {  // Sample.h:83-134: zeros without a trigger; a voice without a buffer gets zeros on the device
+            if (numCh < 1) { zeros(); break; }
+            op.opcode = OP_SAMPLE; take(std::min(numCh, 2));
+            op.mode = (uint32_t) n.mode | (numCh >= 2 ? 4u : 0u);
+            // VariablePitchLerpReader(float sampleRate, ...): 1 - exp(-1 / (0.01 * sampleRate)) in double, stored as float
+            op.aux0 = fbits((float) (1.0 - std::exp(-1.0 / (0.01 * (double) (float) E.sr_))));
+            for (int k = 0; k < 5; ++k) op.operands.push_back({K_PARAM, n.paramRow + k});
         } break;
 
         case NodeKind::TapIn:
@@ -2153,17 +2251,14 @@ int Engine::compile(Group& g, int nIn, std::shared_ptr<Program>& out) {
         if (n.stateRow < 0) return NO_STATE;
         auto it = smemIndexOfRow.find((uint32_t) n.stateRow);
         if (it != smemIndexOfRow.end()) return it->second;
-        const TypeInfo ti = n.kind == NodeKind::Custom ? TypeInfo{NodeKind::Custom, n.fn, customTypes_[n.fn].nState, false} : typeTable().at(n.typeName);
-        if (ti.evenAlign && (nStateRows & 1)) {   // keep doubles 8-byte aligned in shared memory
+        const TypeInfo ti = n.kind == NodeKind::Custom ? TypeInfo{NodeKind::Custom, n.fn, customTypes_[n.fn].nState, 0} : typeTable().at(n.typeName);
+        if (ti.doubleRows > 0 && (nStateRows & 1)) {   // keep doubles 8-byte aligned in shared memory
             prog->stateMap.push_back(STATE_PAD);
             nStateRows += 1;
         }
         const uint32_t idx = (uint32_t) nStateRows;
-        if (ti.evenAlign) {
-            for (int k = 0; k < ti.stateRows; k += 2) prog->stateMap.push_back(((uint32_t) n.stateRow + k) | STATE_DOUBLE_FLAG);
-        } else {
-            for (int k = 0; k < ti.stateRows; ++k) prog->stateMap.push_back((uint32_t) n.stateRow + k);
-        }
+        for (int k = 0; k < ti.doubleRows; k += 2) prog->stateMap.push_back(((uint32_t) n.stateRow + k) | STATE_DOUBLE_FLAG);
+        for (int k = ti.doubleRows; k < ti.stateRows; ++k) prog->stateMap.push_back((uint32_t) n.stateRow + k);
         nStateRows += ti.stateRows;
         smemIndexOfRow[(uint32_t) n.stateRow] = idx;
         return idx;

@@ -33,7 +33,8 @@ enum class NodeKind : uint8_t {
     PassThrough,  // analysis nodes whose events are not produced: audio passes through
     Once, Seq, Seq2, SparSeq, SparSeq2, Time, Metro,  // sequencing / control nodes (SURVEY.md §8f N3)
     Meter, Snapshot, Scope, Capture, Fft,             // analysis nodes feeding processQueuedEvents (SURVEY.md §8f N4)
-    Custom                                            // a device node type registered at run time (registerNodeType)
+    Custom,                                           // a device node type registered at run time (registerNodeType)
+    Sample                                            // sample playback (Sample.h)
 };
 
 // A read-only device array owned jointly by the node that uploaded it and by every compiled program that points at it
@@ -81,10 +82,10 @@ struct Node {
     std::vector<Inlet> inlets;
     std::map<std::string, Value> props;
 
-    int paramRow = -1;               // const / sr: per-voice parameter row
+    int paramRow = -1;               // const / sr: per-voice parameter row; sample: the first of five (ctl_sample, render_kernel.cu)
     int stateRow = -1;               // first scalar state row (even-aligned when it holds doubles)
     int shadowRow = -1;              // rand / once: the seed / arm last set for each voice, outside the state rows (resetVoices)
-    int mode = 0;                    // svf / svfshelf / mm1p mode
+    int mode = 0;                    // svf / svfshelf / mm1p / sample mode
     int channel = 0;                 // in.channel, root.channel (-1 default for root)
     GainFade fade;                   // root
     int size = 0, length = 0;        // delay / sdelay
@@ -96,6 +97,7 @@ struct Node {
     std::string tapName;
     float* tapPrivate = nullptr;     // tapOut private delayBuffer
     std::shared_ptr<Resource> resource;   // table / convolve
+    std::vector<std::shared_ptr<Resource>> voiceRes;   // sample: the buffer each voice of the group plays (kept alive while it does)
     bool resourceDirty = false;
     std::shared_ptr<ConvolverState> conv;
     // seq / seq2 / sparseq / sparseq2 (Core.h:411-466, Seq2.h:39-84, SparSeq.h:40-124, SparSeq2.h:20-56)
@@ -202,19 +204,21 @@ public:
     // count): nProps copies straight from the caller's table, no per-value conversion, no JSON.
     int applyBinary(int voiceBegin, int voiceEnd, const void* data, size_t bytes);
     int setConstTable(const int32_t* nodeIds, int nProps, const float* values, int voiceBegin, int count);
-    // Per-voice `path` of a convolve node: voice voiceBegin+i convolves with the shared resource names[index[i]] from the next block
-    // on, restarting from silence like a [3, nodeId, "path", name] batch on that voice alone — but the voice group is not cut: the
-    // group's K3 state holds one IR per channel (convolve.h).  Everything is checked before anything changes.
+    // Per-voice `path` of a convolve or sample node: voice voiceBegin+i convolves with / plays the shared resource names[index[i]] from
+    // the next block on, restarting from silence like a [3, nodeId, "path", name] batch on that voice alone — but the voice group is not
+    // cut: the group's K3 state holds one IR per channel (convolve.h), a sample node reads its buffer from per-voice parameter rows.
+    // Everything is checked before anything changes.
     int setPathPerVoice(int32_t nodeId, const char* const* names, int numNames, const int32_t* index, int voiceBegin, int count);
     int addSharedResource(const char* name, const float* const* chans, size_t nCh, size_t nSamples);
     void pruneSharedResources();
     std::vector<std::string> listSharedResources() const;
     int gc(int voice, std::vector<int32_t>& pruned);
-    void reset();
     // Voices voices[0..count) (runtime-global, any order, repeats allowed) restart as fresh instances from the next block on: state rows
     // at their creation values (rand / once replayed from their shadow rows), their lanes of every tile buffer and their convolver
     // regions zeroed, pending readouts and capture relays dropped.  One K6 launch, stream-ordered; no group is cut, nothing compiled.
     int resetVoices(const int32_t* voices, size_t count);
+    // Runtime::reset(): every sample node of every voice sends noteOff to both readers (Sample.h:78-81), stream-ordered.
+    void reset();
 
     // Runtime::process shape: planar host buffers; inputs broadcast to every voice; out = mix bus.
     int process(const float* const* in, size_t nIn, float* const* out, size_t nOut, size_t numSamples, const int64_t* sampleTime = nullptr);
@@ -484,6 +488,7 @@ private:
     int fillRow(Group& g, int row, int vb, int ve, float value);
     int fillRowBits(Group& g, int row, int vb, int ve, uint32_t bits);
     int ensureResourceOnDevice(Resource& r);
+    int assignSampleBuffers(Group& g, Node& n, const std::vector<std::shared_ptr<Resource>>& res, const int32_t* index, int vb, int ve);
     int uploadArray(std::shared_ptr<DeviceArray>& out, const void* data, size_t bytes, size_t count);
 
     // compile (Runtime.h:521-577 + GraphRenderSequence.h:107-187)

@@ -72,6 +72,11 @@ enum Opcode : uint32_t {
                    // only in a kernel specialised for the program (spec_host.h): the body text is compiled by NVRTC
     OP_COUNT_
 };
+// Sample playback (Sample.h; render_kernel.cu ctl_sample), numbered after every opcode above and kept out of their enum, which is the
+// set the K1 node-family matrix must cover: `sample` is covered by its own per-voice scenarios instead (DESIGN.md §4).
+// mode = 0 trigger / 1 gate / 2 loop | 4 with a rate child; aux0 = bits of the gain smoother's alpha; operands: trigger, [rate],
+// parameter rows buffer pointer lo / hi, length + 1, startOffset, stopOffset.
+constexpr uint32_t OP_SAMPLE = OP_COUNT_;
 
 // Chain step function codes (one table for the unary, binary and reducing node families of Math.h).
 enum ChainFn : uint32_t {

@@ -507,6 +507,76 @@ __device__ __noinline__ void ctl_capture(const CtlCtx& c) {
     }
     ST(0) = last; ST(1) = __uint_as_float(ssize); ST(2) = __uint_as_float(w); ST(3) = __uint_as_float(r); ST(4) = __uint_as_float(ready);
 }
+
+// Sample.h — SampleNode with its two VariablePitchLerpReaders.  state rows: 0-1 reader 0 pos (double), 2-3 reader 1 pos (double),
+// 4 reader 0 targetGain, 5 reader 0 gain, 6 reader 1 targetGain, 7 reader 1 gain, 8 change.lastIn, 9 currentReader (u32: only its
+// parity is read).  operands: trigger, [rate], then five parameter rows of the voice: buffer pointer low / high word, length + 1
+// (0 = no buffer), startOffset, stopOffset (u32 bits).  mode: 0 trigger / 1 gate / 2 loop, | 4 with a rate child.  aux0 = bits of the
+// gain smoother's alpha.  A read index still outside the buffer after its one wrap, or a position that is NaN or past 2^64, makes the
+// reader output 0 for that sample where the reference reads out of bounds (DESIGN.md §4); its state advances as usual.
+template <int L, int E>
+__device__ __noinline__ void ctl_sample(const CtlCtx& c) {
+    const uint32_t pm = c.mode & 3u;
+    const bool hasRate = (c.mode & 4u) != 0;
+    const Opnd x = ctl_decode<L, E>(c, __ldg(c.opnds));
+    const Opnd r = ctl_decode<L, E>(c, hasRate ? __ldg(c.opnds + 1) : make_operand(K_PARAM, 0));
+    const uint32_t* pw = c.opnds + (hasRate ? 2 : 1);
+    auto par = [&](int i) { return __float_as_uint(c.spar[(int) (__ldg(pw + i) & 0x3FFFFFFFu) * L + c.vlane]); };
+    const uint32_t lenp1 = par(2);
+    if (lenp1 == 0) {                                    // no buffer: zeros, and the edge detector is not fed (Sample.h:101-103)
+        for (int t = 0; t < c.cnt; ++t) c.outT[t * L] = 0.0f;
+        return;
+    }
+    const float* buf = reinterpret_cast<const float*>((uint64_t) par(0) | ((uint64_t) par(1) << 32));
+    const unsigned long long len = lenp1 - 1u, ostart = par(3), ostop = par(4);
+    const double endPos = (double) (len - ostop);        // size_t arithmetic: wraps when stopOffset > length
+    const double startPos = (double) ostart;            // where a loop restarts (Sample.h:193)
+    const double onPos = (double) (float) ostart;       // noteOn: pos = FloatType(startOffset), through float (Sample.h:171)
+    const bool loop = pm == 2u;
+    const float alpha = __uint_as_float(c.aux0);
+    double* pos = reinterpret_cast<double*>(c.sst + c.sidx * L) + c.lane;   // pos[0], pos[L]: the two readers
+    double p0 = pos[0], p1 = pos[L];
+    float tg0 = ST(4), g0 = ST(5), tg1 = ST(6), g1 = ST(7), last = ST(8);
+    uint32_t cur = STU(9);
+    auto tick = [&](double& p, float& g, const float tg, const float rate) -> float {
+        if (p < 0.0 || (g == 0.0f && tg == 0.0f)) return 0.0f;
+        if (p >= endPos) {
+            if (!loop) return 0.0f;
+            p = startPos;
+        }
+        float y = 0.0f;
+        if (p < 18446744073709551616.0) {                // false for NaN too
+            unsigned long long rl = (unsigned long long) p, rr = rl + 1u;
+            const float frac = (float) (p - (double) rl);
+            if (rl >= len) rl -= len;
+            if (rr >= len) rr -= len;
+            if (rl < len && rr < len) {
+                const float left = __ldg(buf + rl), right = __ldg(buf + rr);
+                y = g * (left + frac * (right - left));
+            }
+        }
+        p = p + (double) rate;
+        const float d = tg - g;
+        g = (fabsf(d) <= kEps) ? tg : g + alpha * d;
+        g = clampf(g, 0.0f, 1.0f);
+        return y;
+    };
+    for (int t = 0; t < c.cnt; ++t) {
+        const float cv = change_tick(last, LDT(x, t));
+        const float rate = hasRate ? LDT(r, t) : 1.0f;
+        if (cv > 0.5f) {                                 // rising edge: the current reader fades out, the next one starts
+            if (cur & 1u) tg1 = 0.0f; else tg0 = 0.0f;
+            ++cur;
+            if (cur & 1u) { tg1 = 1.0f; p1 = onPos; } else { tg0 = 1.0f; p0 = onPos; }
+        }
+        if (cv < -0.5f && pm != 0u) { if (cur & 1u) tg1 = 0.0f; else tg0 = 0.0f; }
+        const float y0 = tick(p0, g0, tg0, rate);
+        const float y1 = tick(p1, g1, tg1, rate);
+        c.outT[t * L] = y0 + y1;
+    }
+    pos[0] = p0; pos[L] = p1;
+    ST(4) = tg0; ST(5) = g0; ST(6) = tg1; ST(7) = g1; ST(8) = last; ST(9) = __uint_as_float(cur);
+}
 #undef ST
 #undef STU
 #undef STI

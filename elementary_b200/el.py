@@ -214,6 +214,12 @@ def convolve(props: Dict[str, Any], x: ElemNode) -> Node:
     return create_node("convolve", props, [x])
 
 
+def sample(props: Dict[str, Any], trigger: ElemNode, rate: Optional[ElemNode] = None) -> Node:
+    """Sample playback (core.ts el.sample): plays the shared resource ``props["path"]`` from each rising edge of
+    ``trigger``, at ``rate`` (1 without it).  Props: ``mode`` "trigger" / "gate" / "loop", ``startOffset``, ``stopOffset``."""
+    return create_node("sample", props, [trigger] if rate is None else [trigger, rate])
+
+
 def blepsaw(rate: ElemNode) -> Node:
     return create_node("blepsaw", {}, [rate])
 

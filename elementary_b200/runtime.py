@@ -216,8 +216,9 @@ class Runtime:
                                                           v.ctypes.data_as(C.POINTER(C.c_double)), int(voice_begin), v.size)
 
     def set_path_per_voice(self, node_id: int, names, index, voice_begin: int = 0) -> int:
-        """Voice ``voice_begin + i`` of convolve node ``node_id`` gets the impulse response ``names[index[i]]`` (shared resources),
-        without cutting its voice group; the addressed voices restart from silence at the next block."""
+        """Voice ``voice_begin + i`` of convolve or sample node ``node_id`` gets the impulse response or sample buffer
+        ``names[index[i]]`` (shared resources), without cutting its voice group; the addressed voices restart from silence at the next
+        block (a sample node keeps its voices' trigger edge detector and current reader)."""
         enc = [n.encode() if isinstance(n, str) else bytes(n) for n in names]
         tab = (C.c_char_p * max(1, len(enc)))(*enc)
         idx = np.ascontiguousarray(np.asarray(index, dtype=np.int32).reshape(-1))
@@ -416,6 +417,7 @@ class Runtime:
         return [buf[i] for i in range(min(n, 65536))]
 
     def reset(self) -> None:
+        """Runtime::reset(): both readers of every `sample` node of every voice get noteOff, as in the reference."""
         self._lib.elem_b200_reset(self._h)
 
     # -- ElementaryAudioProcessor::setCurrentTime (wasm/Main.cpp:232-241) ---------------------------------------------

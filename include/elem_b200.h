@@ -63,18 +63,23 @@ int elem_b200_apply_binary(elem_b200_runtime* rt, int voiceBegin, int voiceEnd, 
 int elem_b200_set_const_table(elem_b200_runtime* rt, const int32_t* nodeIds, int numProps, const float* values, int voiceBegin, int count);
 
 /* Vectorised SET_PROPERTY: values[i] -> voice voiceBegin+i; equivalent to `count` single-voice
- * [[3,nodeId,key,values[i]]] batches (Runtime.h:316-333) without `count` JSON parses. */
+ * [[3,nodeId,key,values[i]]] batches (Runtime.h:316-333) without `count` JSON parses.  Per-voice capable: const `value`,
+ * rand `seed`, sample `startOffset` and `stopOffset`; any other node or key returns InvalidPropertyType (5), a sample offset
+ * whose (int) is negative InvalidPropertyValue (6).  All of it is checked before anything changes: a failed call changes nothing. */
 int elem_b200_set_property_per_voice(elem_b200_runtime* rt, int32_t nodeId, const char* key,
                                      const double* values, int voiceBegin, int count);
 
-/* Per-voice impulse response of a `convolve` node (ConvolutionNode::setProperty("path"), wasm/Convolve.h:34-56).
+/* Per-voice impulse response of a `convolve` node (ConvolutionNode::setProperty("path"), wasm/Convolve.h:34-56), or per-voice
+ * buffer of a `sample` node (SampleNode::setProperty("path"), Sample.h:27-36).
  * voice voiceBegin+i gets the `path` names[index[i]]; same result as `count` single-voice
  * [[3, nodeId, "path", names[index[i]]]] batches, except that no voice group is cut.
  * A names table plus a per-voice index, like elem_b200_set_const_table: a million voices choose among K IRs without a million strings.
- * Each addressed voice restarts from silence (a fresh convolver, even on an unchanged name) at the next process/enqueue_block;
- * the other voices are untouched.  Each resource's partition spectra are computed once, however many voices use it.
+ * Each addressed voice restarts from silence at the next process/enqueue_block, even on an unchanged name: a fresh convolver, or
+ * fresh sample readers (currentReader and the trigger's last value are kept); the other voices are untouched.  Each resource's
+ * partition spectra are computed once, however many voices use it; a resource any sample voice plays stays alive across
+ * elem_b200_prune_shared_resources.
  * Returns -2 for a voice range out of bounds or an index outside [0, numNames), NodeNotFound (2) when a voice group in the range
- * lacks the node, InvalidPropertyType (5) when the node is not a convolve, InvalidPropertyValue (6) when a name is not a shared
+ * lacks the node, InvalidPropertyType (5) when the node is neither a convolve nor a sample, InvalidPropertyValue (6) when a name is not a shared
  * resource.  All of it is checked before anything changes: a failed call changes nothing. */
 int elem_b200_set_path_per_voice(elem_b200_runtime* rt, int32_t nodeId, const char* const* names, int numNames,
                                  const int32_t* index, int voiceBegin, int count);
@@ -216,7 +221,8 @@ int elem_b200_list_shared_resources(elem_b200_runtime* rt, char* buf, size_t cap
 /* Runtime::gc() — Runtime.h:76,221-272.  Collects for the voice group containing `voice`; writes up to `cap`
  * pruned node ids (ascending), returns how many were pruned. */
 int elem_b200_gc(elem_b200_runtime* rt, int voice, int32_t* ids, size_t cap);
-/* Runtime::reset() — Runtime.h:70,449-458 */
+/* Runtime::reset() — Runtime.h:70,449-458: as in the reference, only `sample` nodes react: both readers of every voice get noteOff
+ * (they fade out over 10 ms).  Stream-ordered: applied between the previous and the next block. */
 void elem_b200_reset(elem_b200_runtime* rt);
 /* Runtime::processQueuedEvents(cb) — Runtime.h:64,438-446; relayed like wasm/Main.cpp:220-231.  For every root
  * sub-sequence whose root is active, every event node in render order (GraphRenderSequence.h:189-198): `meter`
