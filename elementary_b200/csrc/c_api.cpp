@@ -82,6 +82,11 @@ int elem_b200_set_path_per_voice(elem_b200_runtime* rt, int32_t nodeId, const ch
     GUARD(rt->engine->setPathPerVoice(nodeId, names, numNames, index, voiceBegin, count));
 }
 
+int elem_b200_set_seq_per_voice(elem_b200_runtime* rt, int32_t nodeId, const char* const* seqs, int numSeqs, const int32_t* index, int voiceBegin, int count) {
+    if ((numSeqs > 0 && !seqs) || (count > 0 && !index)) return eb::rc::BadArgument;
+    GUARD(rt->engine->setSeqPerVoice(nodeId, seqs, numSeqs, index, voiceBegin, count));
+}
+
 int elem_b200_reset_voices(elem_b200_runtime* rt, const int32_t* voices, size_t count) {
     if (count > 0 && !voices) return eb::rc::BadArgument;
     GUARD(rt->engine->resetVoices(voices, count));

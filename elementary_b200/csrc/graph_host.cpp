@@ -227,6 +227,8 @@ static void freeGroupStorage(Group& g, bool plan) {
 Engine::~Engine() {
     dsetdev();
     dsync();
+    for (auto& r : retiredArrays_) cudaEventDestroy(r.first);
+    retiredArrays_.clear();
     for (auto& g : groups_) freeGroupStorage(*g, planOnly_);
     groups_.clear();
     for (auto& kv : resources_) if (kv.second->dChannel0) dfree(kv.second->dChannel0);
@@ -465,6 +467,183 @@ int Engine::uploadArray(std::shared_ptr<DeviceArray>& out, const void* data, siz
     if (!cuda(dmalloc(&a->d, std::max<size_t>(bytes, 16)), "cudaMalloc sequence data")) return rc::CudaError;
     if (bytes && !cuda(dmemcpySync(a->d, data, bytes, cudaMemcpyHostToDevice), "upload sequence data")) return rc::CudaError;
     out = a;   // programs compiled against the previous array keep it alive until they are released
+    return rc::Ok;
+}
+
+// A `seq` value as the device array a node of the seq family reads (ctl_seq / ctl_seq2 / ctl_sparseq / ctl_sparseq2): seq and seq2
+// float[n]; sparseq int32 tickTime[n] then float value[n]; sparseq2 double time[n] then float value[n].  The keyed forms are sorted
+// and keep the FIRST value of a duplicated key, like std::map::insert in the reference (SparSeq.h:111, SparSeq2.h:50).
+static int seqBlob(NodeKind kind, const Value& val, std::vector<char>& blob, size_t& count) {
+    if (!val.isArray()) return rc::InvalidPropertyType;
+    if (kind == NodeKind::Seq || kind == NodeKind::Seq2) {   // Core.h:447-466, Seq2.h:60-84
+        std::vector<float> data;
+        for (auto& e : val.asArray()) {
+            if (!e.isNumber()) return rc::InvalidInstructionFormat;   // the reference throws bad_variant_access here
+            data.push_back((float) e.asNumber());
+        }
+        blob.assign(reinterpret_cast<const char*>(data.data()), reinterpret_cast<const char*>(data.data() + data.size()));
+        count = data.size();
+        return rc::Ok;
+    }
+    const bool sparseq = kind == NodeKind::SparSeq;
+    std::map<double, float> m;   // sparseq: the int32 tick time, exact in a double
+    for (auto& e : val.asArray()) {
+        if (!e.isObject()) return rc::InvalidInstructionFormat;
+        auto& o = e.asObject();
+        auto v = o.find("value"), t = o.find(sparseq ? "tickTime" : "time");
+        if (v == o.end() || t == o.end() || !v->second.isNumber() || !t->second.isNumber()) return rc::InvalidInstructionFormat;
+        m.insert({sparseq ? (double) static_cast<int32_t>(t->second.asNumber()) : t->second.asNumber(), (float) v->second.asNumber()});
+    }
+    const size_t kb = sparseq ? 4 : 8;
+    blob.assign(m.size() * (kb + 4), 0);
+    size_t i = 0;
+    for (auto& kv : m) {
+        if (sparseq) { const int32_t t = (int32_t) kv.first; std::memcpy(blob.data() + 4 * i, &t, 4); }
+        else std::memcpy(blob.data() + 8 * i, &kv.first, 8);
+        std::memcpy(blob.data() + kb * m.size() + 4 * i, &kv.second, 4);
+        ++i;
+    }
+    count = m.size();
+    return rc::Ok;
+}
+
+static bool isSeqFamily(NodeKind k) { return k == NodeKind::Seq || k == NodeKind::Seq2 || k == NodeKind::SparSeq || k == NodeKind::SparSeq2; }
+
+// Whether some voice of the group has a non-empty sequence: seq, seq2 and sparseq2 render zeros without touching their state otherwise
+static bool anySeq(const Node& n) {
+    if (n.paramRow < 0) return n.seqData && n.seqData->count > 0;
+    return std::any_of(n.voiceSeq.begin(), n.voiceSeq.end(), [](const std::shared_ptr<DeviceArray>& a) { return a && a->count > 0; });
+}
+
+// [3, id, "seq", val] on group voices [vb, ve) — the whole group: a batch that sets `seq` cuts the group at its voice range first
+int Engine::setGroupSeq(Group& g, Node& n, const Value& val, int vb, int ve) {
+    std::vector<char> blob;
+    size_t count = 0;
+    int r = seqBlob(n.kind, val, blob, count);
+    if (r != rc::Ok) return r;
+    if ((r = uploadArray(n.seqData, blob.data(), blob.size(), count)) != rc::Ok) return r;
+    ++n.seqGen; g.codeDirty = true;
+    if (n.paramRow < 0) return rc::Ok;
+    const std::vector<int32_t> index((size_t) (ve - vb), 0);   // the voices' own rows all take the new sequence
+    return assignSeqRows(g, n, {n.seqData}, index.data(), vb, ve);
+}
+
+// The first per-voice sequence of seq-family node n: four parameter rows (data pointer low / high word, count, generation), filled with
+// the group-wide sequence for every voice.  The next compile sets the op's mode bit 3, which makes it read them.
+int Engine::ensureSeqRows(Group& g, Node& n) {
+    if (n.paramRow >= 0) return rc::Ok;
+    int row = -1;
+    int r = allocRows(g, 4, false, row);
+    if (r != rc::Ok) return r;
+    const uint64_t p = n.seqData ? (uint64_t) (uintptr_t) n.seqData->d : 0;
+    const uint32_t words[4] = {(uint32_t) p, (uint32_t) (p >> 32), n.seqData ? (uint32_t) n.seqData->count : 0u, n.seqGen};
+    for (int k = 0; k < 4; ++k)
+        if ((r = fillRowBits(g, row + k, 0, g.nv, words[k])) != rc::Ok) return r;
+    n.paramRow = row;
+    n.voiceSeq.assign((size_t) g.nv, n.seqData);
+    g.codeDirty = true;
+    return rc::Ok;
+}
+
+// Voice vb + i (group-relative) of seq-family node n reads arrs[index[i]] with generation n.seqGen from its next block on.
+int Engine::assignSeqRows(Group& g, Node& n, const std::vector<std::shared_ptr<DeviceArray>>& arrs, const int32_t* index, int vb, int ve) {
+    const int cnt = ve - vb;
+    if (cnt <= 0) return rc::Ok;
+    std::vector<uint32_t> words((size_t) 4 * cnt);
+    for (int i = 0; i < cnt; ++i) {
+        const DeviceArray& a = *arrs[(size_t) index[i]];
+        const uint64_t p = (uint64_t) (uintptr_t) a.d;
+        words[(size_t) i] = (uint32_t) p;
+        words[(size_t) cnt + i] = (uint32_t) (p >> 32);
+        words[(size_t) 2 * cnt + i] = (uint32_t) a.count;
+        words[(size_t) 3 * cnt + i] = n.seqGen;
+    }
+    for (int k = 0; k < 4; ++k)   // pageable source: staged before the call returns
+        if (!cuda(dmemcpy(g.dRows + (size_t) (n.paramRow + k) * g.Vpad + vb, words.data() + (size_t) k * cnt, sizeof(uint32_t) * cnt, cudaMemcpyHostToDevice), "sequence rows")) return rc::CudaError;
+    if (n.voiceSeq.size() < (size_t) g.nv) n.voiceSeq.resize((size_t) g.nv);
+    std::vector<std::shared_ptr<DeviceArray>> old(n.voiceSeq.begin() + vb, n.voiceSeq.begin() + ve);
+    for (int i = 0; i < cnt; ++i) n.voiceSeq[(size_t) (vb + i)] = arrs[(size_t) index[i]];
+    retireArrays(std::move(old));
+    steadyValid_ = false;
+    return rc::Ok;
+}
+
+// Sequence arrays voices stopped reading.  No program pins them and no later block reads them, but blocks already enqueued may: each is
+// released (freed when nothing else holds it) once the stream has passed an event recorded now.  Stream-ordered deferral, no drain.
+void Engine::retireArrays(std::vector<std::shared_ptr<DeviceArray>>&& arrs) {
+    while (!retiredArrays_.empty() && cudaEventQuery(retiredArrays_.front().first) == cudaSuccess) {
+        cudaEventDestroy(retiredArrays_.front().first);
+        retiredArrays_.pop_front();
+    }
+    std::sort(arrs.begin(), arrs.end());
+    arrs.erase(std::unique(arrs.begin(), arrs.end()), arrs.end());
+    if (!arrs.empty() && !arrs.front()) arrs.erase(arrs.begin());
+    if (planOnly_ || arrs.empty()) return;
+    cudaEvent_t ev = nullptr;
+    if (cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess || cudaEventRecord(ev, stream_) != cudaSuccess) {
+        if (ev) cudaEventDestroy(ev);
+        dsync();   // no event: wait for the blocks instead
+        return;
+    }
+    retiredArrays_.emplace_back(ev, std::move(arrs));
+}
+
+int Engine::setSeqPerVoice(int32_t nodeId, const char* const* seqs, int numSeqs, const int32_t* index, int vb, int count) {
+    // Each distinct text is parsed once, outside the lock, like applyInstructions' batch
+    std::vector<Value> vals((size_t) std::max(0, numSeqs));
+    std::vector<char> parsed(vals.size(), 0);
+    for (size_t k = 0; k < vals.size(); ++k) {
+        if (!seqs[k]) continue;
+        try { vals[k] = parseJson(seqs[k], std::strlen(seqs[k])); parsed[k] = 1; } catch (const std::exception&) {}
+    }
+    Lock lk(mu_);
+    dsetdev();
+    if (vb < 0 || count < 0 || numSeqs < 0 || vb > numVoices_ - count) return fail(rc::BadArgument, "voice range out of bounds");
+    for (int i = 0; i < count; ++i)
+        if (index[i] < 0 || index[i] >= numSeqs) return fail(rc::BadArgument, "sequence index out of range");
+    // every check before any change: a failed call changes nothing
+    std::vector<NodeKind> kinds;   // of the node in the groups of the range (cuts keep a node's kind, so normally one)
+    for (auto& gp : groups_) {
+        const Group& g = *gp;
+        if (std::max(vb, g.v0) >= std::min(vb + count, g.v0 + g.nv)) continue;
+        auto it = g.nodes.find(nodeId);
+        if (it == g.nodes.end()) return rc::NodeNotFound;
+        if (!isSeqFamily(it->second.kind)) return fail(rc::InvalidPropertyType, "node is not a seq, seq2, sparseq or sparseq2");
+        if (std::find(kinds.begin(), kinds.end(), it->second.kind) == kinds.end()) kinds.push_back(it->second.kind);
+    }
+    std::vector<std::vector<char>> blobs(kinds.size() * vals.size());
+    std::vector<size_t> counts(blobs.size(), 0);
+    for (size_t k = 0; k < vals.size(); ++k) {
+        if (!parsed[k]) return fail(rc::InvalidInstructionFormat, "sequence " + std::to_string(k) + " is not valid JSON");
+        for (size_t j = 0; j < kinds.size(); ++j) {
+            const int r = seqBlob(kinds[j], vals[k], blobs[j * vals.size() + k], counts[j * vals.size() + k]);
+            if (r != rc::Ok) return fail(r, "sequence " + std::to_string(k) + " is not a valid seq value for this node");
+        }
+    }
+    if (count == 0) return rc::Ok;
+    // one device array per distinct sequence (and node kind) that some voice takes
+    std::vector<std::vector<std::shared_ptr<DeviceArray>>> arrs(kinds.size(), std::vector<std::shared_ptr<DeviceArray>>(vals.size()));
+    for (size_t j = 0; j < kinds.size(); ++j)
+        for (int i = 0; i < count; ++i) {
+            const size_t k = (size_t) index[i], b = j * vals.size() + k;
+            if (arrs[j][k]) continue;
+            const int r = uploadArray(arrs[j][k], blobs[b].data(), blobs[b].size(), counts[b]);
+            if (r != rc::Ok) return r;
+        }
+    for (auto& gp : groups_) {
+        Group& g = *gp;
+        const int b = std::max(vb, g.v0), e = std::min(vb + count, g.v0 + g.nv);
+        if (b >= e) continue;
+        Node& n = g.nodes.find(nodeId)->second;
+        int r = ensureSeqRows(g, n);
+        if (r != rc::Ok) return r;
+        ++n.seqGen;   // one counter per node, shared with JSON `seq`: a voice's generation changes exactly when it receives a sequence
+        const size_t j = (size_t) (std::find(kinds.begin(), kinds.end(), n.kind) - kinds.begin());
+        const bool had = anySeq(n);
+        if ((r = assignSeqRows(g, n, arrs[j], index + (b - vb), b - g.v0, e - g.v0)) != rc::Ok) return r;
+        if (anySeq(n) != had) g.codeDirty = true;   // the op is emitted while some voice has a sequence
+        n.props["seq"] = vals[(size_t) index[e - 1 - vb]];   // snapshot(): the value last set for the group's highest addressed voice
+    }
     return rc::Ok;
 }
 
@@ -767,17 +946,7 @@ int Engine::nodeSetProperty(Group& g, Node& n, const std::string& key, const Val
                 if (val.asNumber() < 0.0) return rc::InvalidPropertyValue;
                 n.seqOffset = static_cast<uint64_t>(val.asNumber()); g.codeDirty = true;
             }
-            if (key == "seq") {
-                if (!val.isArray()) return rc::InvalidPropertyType;
-                std::vector<float> data;
-                for (auto& e : val.asArray()) {
-                    if (!e.isNumber()) return rc::InvalidInstructionFormat;   // the reference throws bad_variant_access here
-                    data.push_back((float) e.asNumber());
-                }
-                int r = uploadArray(n.seqData, data.data(), data.size() * sizeof(float), data.size());
-                if (r != rc::Ok) return r;
-                ++n.seqGen; g.codeDirty = true;
-            }
+            if (key == "seq") { int r = setGroupSeq(g, n, val, vb, ve); if (r != rc::Ok) return r; }
             break;
         case NodeKind::SparSeq:     // SparSeq.h:40-124
             if (key == "offset") {
@@ -802,42 +971,10 @@ int Engine::nodeSetProperty(Group& g, Node& n, const std::string& key, const Val
                 if (val.asNumber() < 0.0) return rc::InvalidPropertyValue;
                 n.tickIntervalSamples = sr_ * val.asNumber(); g.codeDirty = true;
             }
-            if (key == "seq") {   // std::map<int32_t, float>::insert keeps the FIRST value of a duplicated tick time (SparSeq.h:111)
-                if (!val.isArray()) return rc::InvalidPropertyType;
-                std::map<int32_t, float> m;
-                for (auto& e : val.asArray()) {
-                    if (!e.isObject()) return rc::InvalidInstructionFormat;
-                    auto& o = e.asObject();
-                    auto v = o.find("value"), t = o.find("tickTime");
-                    if (v == o.end() || t == o.end() || !v->second.isNumber() || !t->second.isNumber()) return rc::InvalidInstructionFormat;
-                    m.insert({static_cast<int32_t>(t->second.asNumber()), (float) v->second.asNumber()});
-                }
-                std::vector<char> blob(m.size() * 8);
-                size_t i = 0;
-                for (auto& kv : m) { std::memcpy(blob.data() + 4 * i, &kv.first, 4); std::memcpy(blob.data() + 4 * (m.size() + i), &kv.second, 4); ++i; }
-                int r = uploadArray(n.seqData, blob.data(), blob.size(), m.size());
-                if (r != rc::Ok) return r;
-                ++n.seqGen; g.codeDirty = true;
-            }
+            if (key == "seq") { int r = setGroupSeq(g, n, val, vb, ve); if (r != rc::Ok) return r; }
             break;
         case NodeKind::SparSeq2:    // SparSeq2.h:20-56
-            if (key == "seq") {
-                if (!val.isArray()) return rc::InvalidPropertyType;
-                std::map<double, float> m;
-                for (auto& e : val.asArray()) {
-                    if (!e.isObject()) return rc::InvalidInstructionFormat;
-                    auto& o = e.asObject();
-                    auto v = o.find("value"), t = o.find("time");
-                    if (v == o.end() || t == o.end() || !v->second.isNumber() || !t->second.isNumber()) return rc::InvalidInstructionFormat;
-                    m.insert({t->second.asNumber(), (float) v->second.asNumber()});
-                }
-                std::vector<char> blob(m.size() * 12);
-                size_t i = 0;
-                for (auto& kv : m) { std::memcpy(blob.data() + 8 * i, &kv.first, 8); std::memcpy(blob.data() + 8 * m.size() + 4 * i, &kv.second, 4); ++i; }
-                int r = uploadArray(n.seqData, blob.data(), blob.size(), m.size());
-                if (r != rc::Ok) return r;
-                ++n.seqGen; g.codeDirty = true;
-            }
+            if (key == "seq") { int r = setGroupSeq(g, n, val, vb, ve); if (r != rc::Ok) return r; }
             if (key == "interpolate") { if (!val.isNumber()) return rc::InvalidPropertyType; n.interpolate = static_cast<int32_t>(val.asNumber()); g.codeDirty = true; }
             break;
         case NodeKind::Scope:       // Analyzers.h:155-179
@@ -1041,6 +1178,10 @@ int Engine::splitGroupsAt(int v) {
             if (!kv.second.voiceRes.empty()) {   // so do the buffers sample voices play
                 n.voiceRes.assign(kv.second.voiceRes.begin() + std::min<size_t>(cut, kv.second.voiceRes.size()), kv.second.voiceRes.end());
                 kv.second.voiceRes.resize(std::min<size_t>(cut, kv.second.voiceRes.size()));
+            }
+            if (!kv.second.voiceSeq.empty()) {   // and the sequences seq-family voices read (their rows moved with the other rows)
+                n.voiceSeq.assign(kv.second.voiceSeq.begin() + std::min<size_t>(cut, kv.second.voiceSeq.size()), kv.second.voiceSeq.end());
+                kv.second.voiceSeq.resize(std::min<size_t>(cut, kv.second.voiceSeq.size()));
             }
             if (kv.second.ring) {
                 if (!cloneTiles(kv.second.ring, (size_t) kv.second.size * L, &n.ring)) return rc::CudaError;
@@ -1644,6 +1785,12 @@ int Compiler::emitNode(Node& n, int rootIndex) {
     op.state = (n.stateRow >= 0) ? (uint32_t) n.stateRow : NO_STATE;   // rewritten to a smem index later
     auto zeros = [&]() { op.opcode = OP_FILL0; op.state = NO_STATE; op.operands.clear(); };
     auto take = [&](int k) { op.operands.assign(inputs.begin(), inputs.begin() + k); };
+    // The seq family reads the group's sequence (ptr = data, aux0 = count), or after setSeqPerVoice each voice's own: mode bit 3 and four
+    // parameter rows after the inputs (data pointer low / high word, count, generation).  A voice without a sequence reads count 0.
+    auto seqSource = [&]() {
+        if (n.paramRow >= 0) { op.mode |= 8u; for (int k = 0; k < 4; ++k) op.operands.push_back({K_PARAM, n.paramRow + k}); }
+        else if (n.seqData) { op.aux0 = (uint32_t) n.seqData->count; op.ptr = (uint64_t) (uintptr_t) n.seqData->d; prog.pinned.push_back(n.seqData); }
+    };
 
     switch (n.kind) {
         case NodeKind::In: {   // Math.h:107-122
@@ -1709,31 +1856,29 @@ int Compiler::emitNode(Node& n, int rootIndex) {
         case NodeKind::Once: if (numCh < 1) { zeros(); break; } op.opcode = OP_ONCE; take(1); break;
         case NodeKind::Seq:
         case NodeKind::Seq2: {   // Core.h:497-500, Seq2.h:100-103: zeros without a trigger input or a sequence
-            if (numCh < 1 || !n.seqData || n.seqData->count == 0) { zeros(); break; }
+            if (numCh < 1 || !anySeq(n)) { zeros(); break; }
             op.opcode = n.kind == NodeKind::Seq ? OP_SEQ : OP_SEQ2;
             take(std::min(numCh, 2));
             op.mode = (n.seqHold ? 1u : 0u) | (n.seqLoop ? 2u : 0u) | (numCh > 1 ? 4u : 0u);
-            op.aux0 = (uint32_t) n.seqData->count; op.ptr = (uint64_t) (uintptr_t) n.seqData->d;
+            seqSource();
             op.imm = {(uint32_t) std::min<uint64_t>(n.seqOffset, 0xFFFFFFFFu), n.seqGen};
-            prog.pinned.push_back(n.seqData);
         } break;
         case NodeKind::SparSeq: {   // SparSeq.h:259-262: zeros without a trigger input; the loop-point logic still runs without a sequence
             if (numCh < 1) { zeros(); break; }
             op.opcode = OP_SPARSEQ;
             take(std::min(numCh, 2));
             op.mode = (numCh > 1 ? 4u : 0u);
-            if (n.seqData) { op.aux0 = (uint32_t) n.seqData->count; op.ptr = (uint64_t) (uintptr_t) n.seqData->d; prog.pinned.push_back(n.seqData); }
+            seqSource();
             uint64_t tb; std::memcpy(&tb, &n.tickIntervalSamples, 8);
             op.imm = {(uint32_t) n.seqOffset, n.follow ? 1u : 0u, (uint32_t) n.interpolate, n.seqGen, n.loopGen,
                       (uint32_t) n.loopStart, (uint32_t) n.loopEnd, (uint32_t) tb, (uint32_t) (tb >> 32)};
         } break;
         case NodeKind::SparSeq2: {  // SparSeq2.h:90-91
-            if (numCh < 1 || !n.seqData || n.seqData->count == 0) { zeros(); break; }
+            if (numCh < 1 || !anySeq(n)) { zeros(); break; }
             op.opcode = OP_SPARSEQ2; take(1);
             op.mode = (n.interpolate == 1) ? 1u : 0u;
-            op.aux0 = (uint32_t) n.seqData->count; op.ptr = (uint64_t) (uintptr_t) n.seqData->d;
+            seqSource();
             op.imm = {n.seqGen};
-            prog.pinned.push_back(n.seqData);
         } break;
         case NodeKind::Time: op.opcode = OP_TIME; break;                                     // wasm/SampleTime.h:16-23
         case NodeKind::Metro: op.opcode = OP_METRO; putDouble(op, (double) n.intervalSamps); break;   // wasm/Metro.h:39-55

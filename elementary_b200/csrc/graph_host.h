@@ -5,6 +5,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
+#include <deque>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -82,7 +83,8 @@ struct Node {
     std::vector<Inlet> inlets;
     std::map<std::string, Value> props;
 
-    int paramRow = -1;               // const / sr: per-voice parameter row; sample: the first of five (ctl_sample, render_kernel.cu)
+    int paramRow = -1;               // const / sr: per-voice parameter row; sample: the first of five (ctl_sample, render_kernel.cu);
+                                     // seq family: the first of four, made by the first setSeqPerVoice (ctl_seq_src, render_kernel.cu)
     int stateRow = -1;               // first scalar state row (even-aligned when it holds doubles)
     int shadowRow = -1;              // rand / once: the seed / arm last set for each voice, outside the state rows (resetVoices)
     int mode = 0;                    // svf / svfshelf / mm1p / sample mode
@@ -102,6 +104,7 @@ struct Node {
     std::shared_ptr<ConvolverState> conv;
     // seq / seq2 / sparseq / sparseq2 (Core.h:411-466, Seq2.h:39-84, SparSeq.h:40-124, SparSeq2.h:20-56)
     std::shared_ptr<DeviceArray> seqData;
+    std::vector<std::shared_ptr<DeviceArray>> voiceSeq;   // with paramRow >= 0: the sequence each voice of the group reads
     uint32_t seqGen = 0, loopGen = 0;
     bool seqHold = false, seqLoop = true, follow = false;
     uint64_t seqOffset = 0;
@@ -209,6 +212,11 @@ public:
     // cut: the group's K3 state holds one IR per channel (convolve.h), a sample node reads its buffer from per-voice parameter rows.
     // Everything is checked before anything changes.
     int setPathPerVoice(int32_t nodeId, const char* const* names, int numNames, const int32_t* index, int voiceBegin, int count);
+    // Per-voice `seq` of a seq, seq2, sparseq or sparseq2 node: voice voiceBegin+i gets the JSON value seqs[index[i]] from its next block
+    // on, like a [3, nodeId, "seq", seqs[index[i]]] batch on that voice alone — but the voice group is not cut: the node reads each voice's
+    // sequence from four per-voice parameter rows.  Each distinct text is parsed and uploaded once.  Everything is checked before
+    // anything changes.
+    int setSeqPerVoice(int32_t nodeId, const char* const* seqs, int numSeqs, const int32_t* index, int voiceBegin, int count);
     int addSharedResource(const char* name, const float* const* chans, size_t nCh, size_t nSamples);
     void pruneSharedResources();
     std::vector<std::string> listSharedResources() const;
@@ -490,6 +498,12 @@ private:
     int ensureResourceOnDevice(Resource& r);
     int assignSampleBuffers(Group& g, Node& n, const std::vector<std::shared_ptr<Resource>>& res, const int32_t* index, int vb, int ve);
     int uploadArray(std::shared_ptr<DeviceArray>& out, const void* data, size_t bytes, size_t count);
+    int setGroupSeq(Group& g, Node& n, const Value& val, int vb, int ve);
+    int ensureSeqRows(Group& g, Node& n);
+    int assignSeqRows(Group& g, Node& n, const std::vector<std::shared_ptr<DeviceArray>>& arrs, const int32_t* index, int vb, int ve);
+    void retireArrays(std::vector<std::shared_ptr<DeviceArray>>&& arrs);
+    // sequence arrays no voice reads any more, each batch released once the stream has passed its event (retireArrays)
+    std::deque<std::pair<cudaEvent_t, std::vector<std::shared_ptr<DeviceArray>>>> retiredArrays_;
 
     // compile (Runtime.h:521-577 + GraphRenderSequence.h:107-187)
     int compile(Group& g, int nIn, std::shared_ptr<Program>& out);

@@ -60,6 +60,8 @@ enum Opcode : uint32_t {
     OP_SEQ2,       // Seq2.h:35-166   (same encoding, no generation)
     OP_SPARSEQ,    // SparSeq.h:17-377 (ptr = int32 tickTime[aux0] then float value[aux0]; imm block see graph_host.cpp)
     OP_SPARSEQ2,   // SparSeq2.h:17-141 (ptr = double time[aux0] then float value[aux0]; imm: generation; mode bit0 interpolate)
+                   // the four seq ops, mode bit3: each voice's own sequence from four parameter operands after the inputs (data pointer
+                   // low / high word, count, generation; Engine::setSeqPerVoice), ptr / aux0 / the generation in imm unused
     OP_TIME,       // wasm/SampleTime.h:12-24 (LaunchParams::sampleTime)
     OP_METRO,      // wasm/Metro.h:10-71 ((aux0,aux1) = bits of double(intervalSamps))
     // ---- analysis nodes (SURVEY.md §8f N4): audio passes through, a per-voice record feeds processQueuedEvents ----

@@ -275,22 +275,47 @@ __device__ __noinline__ void ctl_once(const CtlCtx& c) {
     ST(0) = armed; ST(1) = gain; ST(2) = last; ST(3) = isArmed;
 }
 
+// The sequence a seq-family op reads for this voice: the group's (ptr, aux0 = count, the generation in its immediates), or with mode
+// bit 3 the voice's own from the four parameter rows after its nIn inputs: data pointer low / high word, count, generation
+// (Engine::setSeqPerVoice).  A voice whose count is 0 gets zeros from the op, its state untouched, like a group without a sequence.
+// The generation is read only where the op compares it, at the top of a process() call.
+struct SeqSrc { uint64_t ptr; uint32_t n; };
+template <int L>
+__device__ __forceinline__ uint32_t ctl_seq_row(const CtlCtx& c, int nIn, int i) {
+    return __float_as_uint(c.spar[(int) (__ldg(c.opnds + nIn + i) & 0x3FFFFFFFu) * L + c.vlane]);
+}
+template <int L>
+__device__ __forceinline__ SeqSrc ctl_seq_src(const CtlCtx& c, int nIn) {
+    if (!(c.mode & 8u)) return SeqSrc{c.ptr, c.aux0};
+    return SeqSrc{(uint64_t) ctl_seq_row<L>(c, nIn, 0) | ((uint64_t) ctl_seq_row<L>(c, nIn, 1) << 32), ctl_seq_row<L>(c, nIn, 2)};
+}
+template <int L>
+__device__ __forceinline__ uint32_t ctl_seq_gen(const CtlCtx& c, int nIn, const uint32_t* immGen) {
+    return (c.mode & 8u) ? ctl_seq_row<L>(c, nIn, 3) : __ldg(immGen);
+}
+
 // Core.h:407-573 — SequenceNode.  state: change.lastIn, resetChange.lastIn, holdValue, seqIndex, hasReceivedFirstPulse,
-// generation of the sequence data last seen.  imm: [offset, generation].  mode: 1 hold, 2 loop, 4 reset input present.
+// generation of the sequence data last seen.  imm: [offset, generation].  mode: 1 hold, 2 loop, 4 reset input present, 8 the voice's
+// own sequence (ctl_seq_src).
 template <int L, int E>
 __device__ __noinline__ void ctl_seq(const CtlCtx& c) {
     const Opnd x = ctl_decode<L, E>(c, __ldg(c.opnds));
     const bool hasReset = (c.mode & 4u) != 0, hold = (c.mode & 1u) != 0, loop = (c.mode & 2u) != 0;
     const Opnd r = ctl_decode<L, E>(c, hasReset ? __ldg(c.opnds + 1) : make_operand(K_PARAM, 0));
-    const uint32_t offset = __ldg(c.opnds + c.nopnd), codeGen = __ldg(c.opnds + c.nopnd + 1);
-    const float* data = reinterpret_cast<const float*>(c.ptr);
-    const uint32_t n = c.aux0;
+    const SeqSrc src = ctl_seq_src<L>(c, hasReset ? 2 : 1);
+    if (src.n == 0) { for (int t = 0; t < c.cnt; ++t) c.outT[t * L] = 0.0f; return; }
+    const uint32_t offset = __ldg(c.opnds + c.nopnd);
+    const float* data = reinterpret_cast<const float*>(src.ptr);
+    const uint32_t n = src.n;
     float last = ST(0), rlast = ST(1), holdv = ST(2);
     uint32_t idx = STU(3), first = STU(4), gen = STU(5);
-    if (c.s0 == 0 && gen != codeGen) {                   // a new sequence was popped from the queue: Core.h:473-495
-        idx = idx % n;
-        if (first) holdv = __ldg(data + idx);
-        gen = codeGen;
+    if (c.s0 == 0) {
+        const uint32_t codeGen = ctl_seq_gen<L>(c, hasReset ? 2 : 1, c.opnds + c.nopnd + 1);
+        if (gen != codeGen) {                            // a new sequence was popped from the queue: Core.h:473-495
+            idx = idx % n;
+            if (first) holdv = __ldg(data + idx);
+            gen = codeGen;
+        }
     }
     for (int t = 0; t < c.cnt; ++t) {
         const float in = LDT(x, t);
@@ -307,15 +332,17 @@ __device__ __noinline__ void ctl_seq(const CtlCtx& c) {
     ST(3) = __uint_as_float(idx); ST(4) = __uint_as_float(first); ST(5) = __uint_as_float(gen);
 }
 
-// Seq2.h:87-148 — Seq2Node.  state: change.lastIn, resetChange.lastIn, edgeCount.  imm: [offset].
+// Seq2.h:87-148 — Seq2Node.  state: change.lastIn, resetChange.lastIn, edgeCount.  imm: [offset].  mode as ctl_seq's.
 template <int L, int E>
 __device__ __noinline__ void ctl_seq2(const CtlCtx& c) {
     const Opnd x = ctl_decode<L, E>(c, __ldg(c.opnds));
     const bool hasReset = (c.mode & 4u) != 0, hold = (c.mode & 1u) != 0, loop = (c.mode & 2u) != 0;
     const Opnd r = ctl_decode<L, E>(c, hasReset ? __ldg(c.opnds + 1) : make_operand(K_PARAM, 0));
+    const SeqSrc src = ctl_seq_src<L>(c, hasReset ? 2 : 1);
+    if (src.n == 0) { for (int t = 0; t < c.cnt; ++t) c.outT[t * L] = 0.0f; return; }
     const unsigned long long offset = __ldg(c.opnds + c.nopnd);
-    const float* data = reinterpret_cast<const float*>(c.ptr);
-    const unsigned long long n = c.aux0;
+    const float* data = reinterpret_cast<const float*>(src.ptr);
+    const unsigned long long n = src.n;
     float last = ST(0), rlast = ST(1);
     uint32_t edge = STU(2);
     for (int t = 0; t < c.cnt; ++t) {
@@ -343,18 +370,22 @@ __device__ __forceinline__ int upper_bound_idx(const K* keys, int n, K t) {
 }
 
 // SparSeq2.h:69-128 — SparSeq2Node.  ptr = double time[n] then float value[n].  state: prevEvent, nextEvent (indices, n =
-// end()), generation.  imm: [generation].  mode bit0 = interpolate.
+// end()), generation.  imm: [generation].  mode bit0 = interpolate, bit3 the voice's own sequence (ctl_seq_src).
 template <int L, int E>
 __device__ __noinline__ void ctl_sparseq2(const CtlCtx& c) {
     const Opnd x = ctl_decode<L, E>(c, __ldg(c.opnds));
-    const int n = (int) c.aux0;
-    const double* times = reinterpret_cast<const double*>(c.ptr);
+    const SeqSrc src = ctl_seq_src<L>(c, 1);
+    if (src.n == 0) { for (int t = 0; t < c.cnt; ++t) c.outT[t * L] = 0.0f; return; }
+    const int n = (int) src.n;
+    const double* times = reinterpret_cast<const double*>(src.ptr);
     const float* values = reinterpret_cast<const float*>(times + n);
     const bool interp = (c.mode & 1u) != 0;
-    const uint32_t codeGen = __ldg(c.opnds + c.nopnd);
     int prev = STI(0), next = STI(1);
     uint32_t gen = STU(2);
-    if (c.s0 == 0 && gen != codeGen) { prev = n; next = n; gen = codeGen; }   // SparSeq2.h:77-86
+    if (c.s0 == 0) {
+        const uint32_t codeGen = ctl_seq_gen<L>(c, 1, c.opnds + c.nopnd);
+        if (gen != codeGen) { prev = n; next = n; gen = codeGen; }   // SparSeq2.h:77-86
+    }
     for (int i = 0; i < c.cnt; ++i) {
         const double t = (double) LDT(x, i);
         const bool update = (prev == n && next == n) || (prev != n && t <= (times[prev] + 1e-9)) || (next != n && t >= (times[next] - 1e-9));
@@ -377,7 +408,8 @@ __device__ __noinline__ void ctl_sparseq2(const CtlCtx& c) {
 // SparSeq.h:17-377 — SparSeqNode.  ptr = int32 tickTime[n] then float value[n] (0 = no sequence yet).
 // state rows: 0 change.lastIn, 1 resetChange.lastIn, 2 edgeCount, 3 samplesSinceClockEdge, 4 holdValue (index, n = end()),
 // 5/6 loopPoints, 7 pending flag, 8/9 pendingLoopPoints, 10 sequence generation seen, 11 loop-points generation seen,
-// 12 tickTime (a local of process(), carried between the sample tiles of one call).
+// 12 tickTime (a local of process(), carried between the sample tiles of one call).  mode: 4 reset input present, 8 the voice's own
+// sequence (ctl_seq_src).
 // imm: [offset, follow, interpolate, seqGen, loopGen, loopStart, loopEnd, tickInterval lo, hi].
 struct SparSeqState { int edge, ls, le, pend, ps, pe; };
 
@@ -415,12 +447,12 @@ __device__ __noinline__ void ctl_sparseq(const CtlCtx& c) {
     const Opnd r = ctl_decode<L, E>(c, hasReset ? __ldg(c.opnds + 1) : make_operand(K_PARAM, 0));
     const uint32_t* imm = c.opnds + c.nopnd;
     const int offset = (int) __ldg(imm), follow = (int) __ldg(imm + 1), ho = (int) __ldg(imm + 2);
-    const uint32_t seqGen = __ldg(imm + 3), loopGen = __ldg(imm + 4);
-    const double spc = bits_to_double(__ldg(imm + 7), __ldg(imm + 8));
-    const int n = (int) c.aux0;
-    const bool hasSeq = c.ptr != 0;
-    const int* times = reinterpret_cast<const int*>(c.ptr);
-    const float* values = reinterpret_cast<const float*>(times + n);
+    const SeqSrc src = ctl_seq_src<L>(c, hasReset ? 2 : 1);
+    const uint32_t loopGen = __ldg(imm + 4);
+    const int n = (int) src.n;
+    const bool hasSeq = src.ptr != 0;     // an empty sequence still counts edges (SparSeq.h:259-262)
+    const int* times = reinterpret_cast<const int*>(src.ptr);
+    auto values = [&](int i) { return __int_as_float(times[n + i]); };   // value[i] follows the n tick times
 
     float last = ST(0), rlast = ST(1);
     SparSeqState s{STI(2), STI(5), STI(6), STI(7), STI(8), STI(9)};
@@ -428,6 +460,7 @@ __device__ __noinline__ void ctl_sparseq(const CtlCtx& c) {
     int holdIdx = STI(4), tick = STI(12);
     if (c.s0 == 0) {                                       // top of process(): SparSeq.h:209-257
         tick = sparseq_tick_time(s, offset);
+        const uint32_t seqGen = ctl_seq_gen<L>(c, hasReset ? 2 : 1, imm + 3);
         uint32_t sg = STU(10), lg = STU(11);
         if (sg != seqGen || lg != loopGen) {
             if (lg != loopGen) { s.pend = 1; s.ps = (int) __ldg(imm + 5); s.pe = (int) __ldg(imm + 6); }
@@ -459,15 +492,16 @@ __device__ __noinline__ void ctl_sparseq(const CtlCtx& c) {
             if (holdIdx == n) y = 0.0f;
             else if (ho == 1) {
                 const int right = holdIdx + 1;
-                if (right == n) y = values[holdIdx];
+                if (right == n) y = values(holdIdx);
                 else {
                     const int tl = times[holdIdx], tr = times[right];
-                    const float lv = values[holdIdx], rv = values[right];
+                    const float lv = values(holdIdx), rv = values(right);
+                    const double spc = bits_to_double(__ldg(imm + 7), __ldg(imm + 8));
                     double alpha = (double) max(0, tick - tl) / (double) (tr - tl);
                     if (spc > 0.0) alpha += (fmin((double) since, spc) / spc) / (double) (tr - tl);
                     y = (float) ((double) lv + alpha * (double) (rv - lv));
                 }
-            } else y = values[holdIdx];
+            } else y = values(holdIdx);
             c.outT[i * L] = y;
         }
     }

@@ -63,6 +63,8 @@ def load_library() -> C.CDLL:
     lib.elem_b200_set_property_per_voice.argtypes = [C.c_void_p, C.c_int32, C.c_char_p, C.POINTER(C.c_double), C.c_int, C.c_int]
     lib.elem_b200_set_path_per_voice.restype = C.c_int
     lib.elem_b200_set_path_per_voice.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), C.c_int, C.POINTER(C.c_int32), C.c_int, C.c_int]
+    lib.elem_b200_set_seq_per_voice.restype = C.c_int
+    lib.elem_b200_set_seq_per_voice.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), C.c_int, C.POINTER(C.c_int32), C.c_int, C.c_int]
     lib.elem_b200_reset_voices.restype = C.c_int
     lib.elem_b200_reset_voices.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_size_t]
     lib.elem_b200_reset_bytes_written.restype = C.c_uint64
@@ -224,6 +226,17 @@ class Runtime:
         idx = np.ascontiguousarray(np.asarray(index, dtype=np.int32).reshape(-1))
         return self._lib.elem_b200_set_path_per_voice(self._h, int(node_id), tab, len(enc),
                                                       idx.ctypes.data_as(C.POINTER(C.c_int32)), int(voice_begin), idx.size)
+
+    def set_seq_per_voice(self, node_id: int, seqs, index, voice_begin: int = 0) -> int:
+        """Voice ``voice_begin + i`` of seq, seq2, sparseq or sparseq2 node ``node_id`` gets the sequence ``seqs[index[i]]`` (a Python
+        value such as ``[1, 2, 3]`` or ``[{"tickTime": 0, "value": 1}]``, JSON-encoded here; bytes pass through as JSON text),
+        without cutting its voice group: the same as single-voice ``[3, node_id, "seq", seqs[index[i]]]`` batches.  Each distinct
+        sequence is parsed and uploaded once."""
+        enc = [s if isinstance(s, bytes) else json.dumps(s).encode() for s in seqs]
+        tab = (C.c_char_p * max(1, len(enc)))(*enc)
+        idx = np.ascontiguousarray(np.asarray(index, dtype=np.int32).reshape(-1))
+        return self._lib.elem_b200_set_seq_per_voice(self._h, int(node_id), tab, len(enc),
+                                                     idx.ctypes.data_as(C.POINTER(C.c_int32)), int(voice_begin), idx.size)
 
     def reset_voices(self, voices) -> int:
         """The given voices (runtime-global indices, any order, repeats allowed) restart as fresh instances from the next block on, as

@@ -84,6 +84,21 @@ int elem_b200_set_property_per_voice(elem_b200_runtime* rt, int32_t nodeId, cons
 int elem_b200_set_path_per_voice(elem_b200_runtime* rt, int32_t nodeId, const char* const* names, int numNames,
                                  const int32_t* index, int voiceBegin, int count);
 
+/* Per-voice sequence of a `seq`, `seq2`, `sparseq` or `sparseq2` node (their setProperty("seq"), Core.h:447-466, Seq2.h:60-84,
+ * SparSeq.h:102-124, SparSeq2.h:39-56).  seqs[k] is the JSON text of one `seq` value, as [3, nodeId, "seq", value] carries it; voice
+ * voiceBegin+i gets seqs[index[i]].  Same result as `count` single-voice [[3, nodeId, "seq", seqs[index[i]]]] batches, except that no
+ * voice group is cut: the node reads each voice's sequence from per-voice parameter rows.  Each addressed voice takes its sequence at
+ * its next block as its own Runtime would, even an unchanged one (seq: index wrapped and hold value reloaded; sparseq: hold index
+ * re-found; sparseq2: previous / next event reset); the other voices are untouched.  Each distinct seqs[k] is parsed and uploaded once,
+ * however many voices use it.  A later whole-group [3, nodeId, "seq", v] gives every voice of the group v; voice resets keep a voice's
+ * sequence; snapshot() reports the value set for the group's highest addressed voice.
+ * Returns -2 for a voice range out of bounds or an index outside [0, numSeqs), NodeNotFound (2) when a voice group in the range lacks
+ * the node, InvalidPropertyType (5) when the node is not one of the four, and for a seqs[k] what [3, nodeId, "seq", seqs[k]] returns
+ * on that node (5 for a non-array, 8 for a malformed entry), 8 for text that is not JSON.  All of it is checked before anything
+ * changes: a failed call changes nothing. */
+int elem_b200_set_seq_per_voice(elem_b200_runtime* rt, int32_t nodeId, const char* const* seqs, int numSeqs,
+                                const int32_t* index, int voiceBegin, int count);
+
 /* Voices voices[0..count) restart as fresh instances: each renders from its next block on what a Runtime newly
  * created and given this runtime's instruction history would render. Props are replayed as last set for that voice.
  * Stream-ordered: applied between the previous and the next block, with no host synchronisation. No voice group is
