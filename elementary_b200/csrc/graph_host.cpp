@@ -156,6 +156,49 @@ static const std::unordered_map<std::string, TypeInfo>& typeTable() {
     return t;
 }
 
+// Per-voice parameter rows after Node::paramRow, as the render kernel reads them: sample (ctl_sample, render_kernel.cu) and the seq
+// family with its voices' own sequences (ctl_seq_src).  Both begin with the array a voice reads (VoiceArray): its device address, low
+// and high word, and a length word — a sample's numSamples + 1 (0: no buffer), a sequence's count.
+constexpr int ARRAY_ROWS = 3;
+constexpr int SAMPLE_START_OFFSET = 3, SAMPLE_STOP_OFFSET = 4, SAMPLE_PARAM_ROWS = 5;
+constexpr int SEQ_GEN = 3, SEQ_PARAM_ROWS = 4;
+// sample state rows (ctl_sample): the two readers' positions (double row pairs), then their target gains and gains, interleaved
+constexpr int SAMPLE_POS0 = 0, SAMPLE_POS1 = 2, SAMPLE_TARGET_GAIN0 = 4, SAMPLE_TARGET_GAIN1 = 6, SAMPLE_GAINS_END = 8;
+
+struct VoiceArray { std::shared_ptr<const void> hold; uint64_t ptr = 0; uint32_t len = 0; };
+// What a per-voice call on voices [vb, vb + count) touches in one voice group: the node, its voices [b, e) there (group-relative), and
+// `at`, the index of voice b in the call's per-voice arrays.  snapshot() reports the value set for voice last(), the highest addressed.
+struct VoiceTarget { Group& g; Node& n; int b, e, at; int last() const { return at + e - b - 1; } };
+static bool voiceRangeOk(int vb, int count, int numVoices) { return vb >= 0 && count >= 0 && vb <= numVoices - count; }   // cannot overflow
+static VoiceArray seqArray(const std::shared_ptr<DeviceArray>& a) {
+    return a ? VoiceArray{a, (uint64_t) (uintptr_t) a->d, (uint32_t) a->count} : VoiceArray{};
+}
+
+// The props a per-voice call may set without cutting the voice group — setPropertyPerVoice, and JSON batches made of nothing else
+// (isValueOnlyBatch): the row a value goes to (n.*base + row, and with `shadow` the node's shadow row) and its row bits.  once.arm is
+// JSON-only, a bool (no bits): it can arm but never disarm, which a table of per-voice values cannot express.
+struct PerVoiceProp {
+    NodeKind kind; const char* key;
+    using NodeRow = int Node::*;
+    NodeRow base; int row; bool shadow;
+    bool (*bits)(double v, uint32_t& out);   // false: the value is invalid (InvalidPropertyValue)
+};
+static bool floatBits(double v, uint32_t& out) { const float f = (float) v; std::memcpy(&out, &f, 4); return true; }
+static bool seedBits(double v, uint32_t& out) { out = static_cast<uint32_t>(v); return true; }
+static bool offsetBits(double v, uint32_t& out) { out = (uint32_t) static_cast<int>(v); return static_cast<int>(v) >= 0; }   // Sample.h:56,69
+static const PerVoiceProp* perVoiceProp(NodeKind kind, const std::string& key) {
+    static const PerVoiceProp props[] = {
+        {NodeKind::Const, "value", &Node::paramRow, 0, false, floatBits},
+        {NodeKind::Rand, "seed", &Node::stateRow, 0, true, seedBits},
+        {NodeKind::Once, "arm", &Node::stateRow, 0, true, nullptr},
+        {NodeKind::Sample, "startOffset", &Node::paramRow, SAMPLE_START_OFFSET, false, offsetBits},
+        {NodeKind::Sample, "stopOffset", &Node::paramRow, SAMPLE_STOP_OFFSET, false, offsetBits},
+    };
+    for (const auto& p : props)
+        if (p.kind == kind && key == p.key) return &p;
+    return nullptr;
+}
+
 // Fresh state, the one definition of what a node holds right after creation: createNode writes it, compile writes a delay's again
 // when its ring is (re)allocated, and resetVoices restores it.  State row k of a node of this kind starts as freshRowBits(kind, k);
 // row shadowedRow(kind) (-1: none) is a prop the reference sets per instance (rand.seed, once.arm), restored from the node's shadow
@@ -227,8 +270,7 @@ static void freeGroupStorage(Group& g, bool plan) {
 Engine::~Engine() {
     dsetdev();
     dsync();
-    for (auto& r : retiredArrays_) cudaEventDestroy(r.first);
-    retiredArrays_.clear();
+    retireArrays({});
     for (auto& g : groups_) freeGroupStorage(*g, planOnly_);
     groups_.clear();
     for (auto& kv : resources_) if (kv.second->dChannel0) dfree(kv.second->dChannel0);
@@ -452,6 +494,39 @@ int Engine::fillRow(Group& g, int row, int vb, int ve, float value) {
     return fillRowBits(g, row, vb, ve, bits);
 }
 
+// Rows row .. row + rows - 1 of group voices [vb, vb + cnt) <- words[k * cnt + i] (32-bit words, row-major).  The source is pageable:
+// staged before the call returns (fillRowBits), so it may die right after.
+int Engine::writeColumns(Group& g, int row, int rows, int vb, int cnt, const void* words, const char* what) {
+    for (int k = 0; k < rows; ++k)
+        if (!cuda(dmemcpy(g.dRows + (size_t) (row + k) * g.Vpad + vb, static_cast<const uint32_t*>(words) + (size_t) k * cnt,
+                          sizeof(uint32_t) * cnt, cudaMemcpyHostToDevice), what)) return rc::CudaError;
+    return rc::Ok;
+}
+
+// Voice vb + i (group-relative, i < ve - vb) of node n reads arrs[index[i]] (index null: arrs[0]) from its next block on: the array's
+// address and length go to the node's first ARRAY_ROWS parameter rows — a seq-family node's generation *gen to the next (SEQ_GEN) —
+// and the voice holds the array.  The arrays the voices held before are retired (retireArrays).
+int Engine::assignVoiceArrays(Group& g, Node& n, const std::vector<VoiceArray>& arrs, const int32_t* index, int vb, int ve, const uint32_t* gen) {
+    const int cnt = ve - vb, rows = gen ? SEQ_PARAM_ROWS : ARRAY_ROWS;
+    if (cnt <= 0) return rc::Ok;
+    std::vector<uint32_t> words((size_t) rows * cnt);
+    for (int i = 0; i < cnt; ++i) {
+        const VoiceArray& a = arrs[index ? (size_t) index[i] : 0];
+        words[(size_t) i] = (uint32_t) a.ptr;
+        words[(size_t) cnt + i] = (uint32_t) (a.ptr >> 32);
+        words[(size_t) 2 * cnt + i] = a.len;
+        if (gen) words[(size_t) SEQ_GEN * cnt + i] = *gen;
+    }
+    const int r = writeColumns(g, n.paramRow, rows, vb, cnt, words.data(), "per-voice array rows");
+    if (r != rc::Ok) return r;
+    if (n.voiceArrays.size() < (size_t) g.nv) n.voiceArrays.resize((size_t) g.nv);
+    std::vector<std::shared_ptr<const void>> old(n.voiceArrays.begin() + vb, n.voiceArrays.begin() + ve);
+    for (int i = 0; i < cnt; ++i) n.voiceArrays[(size_t) (vb + i)] = arrs[index ? (size_t) index[i] : 0].hold;
+    retireArrays(std::move(old));
+    steadyValid_ = false;
+    return rc::Ok;
+}
+
 int Engine::ensureResourceOnDevice(Resource& r) {
     if (r.dChannel0 || r.numSamples == 0) return rc::Ok;
     const size_t padded = (r.numSamples + 3) / 4 * 4;
@@ -512,65 +587,13 @@ static bool isSeqFamily(NodeKind k) { return k == NodeKind::Seq || k == NodeKind
 // Whether some voice of the group has a non-empty sequence: seq, seq2 and sparseq2 render zeros without touching their state otherwise
 static bool anySeq(const Node& n) {
     if (n.paramRow < 0) return n.seqData && n.seqData->count > 0;
-    return std::any_of(n.voiceSeq.begin(), n.voiceSeq.end(), [](const std::shared_ptr<DeviceArray>& a) { return a && a->count > 0; });
+    return std::any_of(n.voiceArrays.begin(), n.voiceArrays.end(),
+                       [](const std::shared_ptr<const void>& a) { return a && static_cast<const DeviceArray*>(a.get())->count > 0; });
 }
 
-// [3, id, "seq", val] on group voices [vb, ve) — the whole group: a batch that sets `seq` cuts the group at its voice range first
-int Engine::setGroupSeq(Group& g, Node& n, const Value& val, int vb, int ve) {
-    std::vector<char> blob;
-    size_t count = 0;
-    int r = seqBlob(n.kind, val, blob, count);
-    if (r != rc::Ok) return r;
-    if ((r = uploadArray(n.seqData, blob.data(), blob.size(), count)) != rc::Ok) return r;
-    ++n.seqGen; g.codeDirty = true;
-    if (n.paramRow < 0) return rc::Ok;
-    const std::vector<int32_t> index((size_t) (ve - vb), 0);   // the voices' own rows all take the new sequence
-    return assignSeqRows(g, n, {n.seqData}, index.data(), vb, ve);
-}
-
-// The first per-voice sequence of seq-family node n: four parameter rows (data pointer low / high word, count, generation), filled with
-// the group-wide sequence for every voice.  The next compile sets the op's mode bit 3, which makes it read them.
-int Engine::ensureSeqRows(Group& g, Node& n) {
-    if (n.paramRow >= 0) return rc::Ok;
-    int row = -1;
-    int r = allocRows(g, 4, false, row);
-    if (r != rc::Ok) return r;
-    const uint64_t p = n.seqData ? (uint64_t) (uintptr_t) n.seqData->d : 0;
-    const uint32_t words[4] = {(uint32_t) p, (uint32_t) (p >> 32), n.seqData ? (uint32_t) n.seqData->count : 0u, n.seqGen};
-    for (int k = 0; k < 4; ++k)
-        if ((r = fillRowBits(g, row + k, 0, g.nv, words[k])) != rc::Ok) return r;
-    n.paramRow = row;
-    n.voiceSeq.assign((size_t) g.nv, n.seqData);
-    g.codeDirty = true;
-    return rc::Ok;
-}
-
-// Voice vb + i (group-relative) of seq-family node n reads arrs[index[i]] with generation n.seqGen from its next block on.
-int Engine::assignSeqRows(Group& g, Node& n, const std::vector<std::shared_ptr<DeviceArray>>& arrs, const int32_t* index, int vb, int ve) {
-    const int cnt = ve - vb;
-    if (cnt <= 0) return rc::Ok;
-    std::vector<uint32_t> words((size_t) 4 * cnt);
-    for (int i = 0; i < cnt; ++i) {
-        const DeviceArray& a = *arrs[(size_t) index[i]];
-        const uint64_t p = (uint64_t) (uintptr_t) a.d;
-        words[(size_t) i] = (uint32_t) p;
-        words[(size_t) cnt + i] = (uint32_t) (p >> 32);
-        words[(size_t) 2 * cnt + i] = (uint32_t) a.count;
-        words[(size_t) 3 * cnt + i] = n.seqGen;
-    }
-    for (int k = 0; k < 4; ++k)   // pageable source: staged before the call returns
-        if (!cuda(dmemcpy(g.dRows + (size_t) (n.paramRow + k) * g.Vpad + vb, words.data() + (size_t) k * cnt, sizeof(uint32_t) * cnt, cudaMemcpyHostToDevice), "sequence rows")) return rc::CudaError;
-    if (n.voiceSeq.size() < (size_t) g.nv) n.voiceSeq.resize((size_t) g.nv);
-    std::vector<std::shared_ptr<DeviceArray>> old(n.voiceSeq.begin() + vb, n.voiceSeq.begin() + ve);
-    for (int i = 0; i < cnt; ++i) n.voiceSeq[(size_t) (vb + i)] = arrs[(size_t) index[i]];
-    retireArrays(std::move(old));
-    steadyValid_ = false;
-    return rc::Ok;
-}
-
-// Sequence arrays voices stopped reading.  No program pins them and no later block reads them, but blocks already enqueued may: each is
-// released (freed when nothing else holds it) once the stream has passed an event recorded now.  Stream-ordered deferral, no drain.
-void Engine::retireArrays(std::vector<std::shared_ptr<DeviceArray>>&& arrs) {
+// Arrays voices stopped reading.  No program pins them and no later block reads them, but blocks already enqueued may: each is released
+// (freed when nothing else holds it) once the stream has passed an event recorded now.  Stream-ordered deferral, no drain.
+void Engine::retireArrays(std::vector<std::shared_ptr<const void>>&& arrs) {
     while (!retiredArrays_.empty() && cudaEventQuery(retiredArrays_.front().first) == cudaSuccess) {
         cudaEventDestroy(retiredArrays_.front().first);
         retiredArrays_.pop_front();
@@ -598,51 +621,47 @@ int Engine::setSeqPerVoice(int32_t nodeId, const char* const* seqs, int numSeqs,
     }
     Lock lk(mu_);
     dsetdev();
-    if (vb < 0 || count < 0 || numSeqs < 0 || vb > numVoices_ - count) return fail(rc::BadArgument, "voice range out of bounds");
+    if (numSeqs < 0) return fail(rc::BadArgument, "voice range out of bounds");
     for (int i = 0; i < count; ++i)
         if (index[i] < 0 || index[i] >= numSeqs) return fail(rc::BadArgument, "sequence index out of range");
     // every check before any change: a failed call changes nothing
+    std::vector<VoiceTarget> targets;
+    int r = voiceTargets(nodeId, vb, count, isSeqFamily, "node is not a seq, seq2, sparseq or sparseq2", targets);
+    if (r != rc::Ok) return r;
     std::vector<NodeKind> kinds;   // of the node in the groups of the range (cuts keep a node's kind, so normally one)
-    for (auto& gp : groups_) {
-        const Group& g = *gp;
-        if (std::max(vb, g.v0) >= std::min(vb + count, g.v0 + g.nv)) continue;
-        auto it = g.nodes.find(nodeId);
-        if (it == g.nodes.end()) return rc::NodeNotFound;
-        if (!isSeqFamily(it->second.kind)) return fail(rc::InvalidPropertyType, "node is not a seq, seq2, sparseq or sparseq2");
-        if (std::find(kinds.begin(), kinds.end(), it->second.kind) == kinds.end()) kinds.push_back(it->second.kind);
-    }
+    for (auto& t : targets)
+        if (std::find(kinds.begin(), kinds.end(), t.n.kind) == kinds.end()) kinds.push_back(t.n.kind);
     std::vector<std::vector<char>> blobs(kinds.size() * vals.size());
     std::vector<size_t> counts(blobs.size(), 0);
     for (size_t k = 0; k < vals.size(); ++k) {
         if (!parsed[k]) return fail(rc::InvalidInstructionFormat, "sequence " + std::to_string(k) + " is not valid JSON");
         for (size_t j = 0; j < kinds.size(); ++j) {
-            const int r = seqBlob(kinds[j], vals[k], blobs[j * vals.size() + k], counts[j * vals.size() + k]);
-            if (r != rc::Ok) return fail(r, "sequence " + std::to_string(k) + " is not a valid seq value for this node");
+            if ((r = seqBlob(kinds[j], vals[k], blobs[j * vals.size() + k], counts[j * vals.size() + k])) != rc::Ok)
+                return fail(r, "sequence " + std::to_string(k) + " is not a valid seq value for this node");
         }
     }
-    if (count == 0) return rc::Ok;
     // one device array per distinct sequence (and node kind) that some voice takes
-    std::vector<std::vector<std::shared_ptr<DeviceArray>>> arrs(kinds.size(), std::vector<std::shared_ptr<DeviceArray>>(vals.size()));
+    std::vector<std::vector<VoiceArray>> arrs(kinds.size(), std::vector<VoiceArray>(vals.size()));
     for (size_t j = 0; j < kinds.size(); ++j)
         for (int i = 0; i < count; ++i) {
             const size_t k = (size_t) index[i], b = j * vals.size() + k;
-            if (arrs[j][k]) continue;
-            const int r = uploadArray(arrs[j][k], blobs[b].data(), blobs[b].size(), counts[b]);
-            if (r != rc::Ok) return r;
+            if (arrs[j][k].hold) continue;
+            std::shared_ptr<DeviceArray> a;
+            if ((r = uploadArray(a, blobs[b].data(), blobs[b].size(), counts[b])) != rc::Ok) return r;
+            arrs[j][k] = seqArray(a);
         }
-    for (auto& gp : groups_) {
-        Group& g = *gp;
-        const int b = std::max(vb, g.v0), e = std::min(vb + count, g.v0 + g.nv);
-        if (b >= e) continue;
-        Node& n = g.nodes.find(nodeId)->second;
-        int r = ensureSeqRows(g, n);
-        if (r != rc::Ok) return r;
-        ++n.seqGen;   // one counter per node, shared with JSON `seq`: a voice's generation changes exactly when it receives a sequence
-        const size_t j = (size_t) (std::find(kinds.begin(), kinds.end(), n.kind) - kinds.begin());
-        const bool had = anySeq(n);
-        if ((r = assignSeqRows(g, n, arrs[j], index + (b - vb), b - g.v0, e - g.v0)) != rc::Ok) return r;
-        if (anySeq(n) != had) g.codeDirty = true;   // the op is emitted while some voice has a sequence
-        n.props["seq"] = vals[(size_t) index[e - 1 - vb]];   // snapshot(): the value last set for the group's highest addressed voice
+    for (auto& t : targets) {
+        if (t.n.paramRow < 0) {   // its first per-voice sequence: the rows, every voice on the group's sequence; the next compile sets mode bit 3
+            if ((r = allocRows(t.g, SEQ_PARAM_ROWS, false, t.n.paramRow)) != rc::Ok ||
+                (r = assignVoiceArrays(t.g, t.n, {seqArray(t.n.seqData)}, nullptr, 0, t.g.nv, &t.n.seqGen)) != rc::Ok) return r;
+            t.g.codeDirty = true;
+        }
+        ++t.n.seqGen;   // one counter per node, shared with JSON `seq`: a voice's generation changes exactly when it receives a sequence
+        const size_t j = (size_t) (std::find(kinds.begin(), kinds.end(), t.n.kind) - kinds.begin());
+        const bool had = anySeq(t.n);
+        if ((r = assignVoiceArrays(t.g, t.n, arrs[j], index + t.at, t.b, t.e, &t.n.seqGen)) != rc::Ok) return r;
+        if (anySeq(t.n) != had) t.g.codeDirty = true;   // the op is emitted while some voice has a sequence
+        t.n.props["seq"] = vals[(size_t) index[t.last()]];
     }
     return rc::Ok;
 }
@@ -663,6 +682,7 @@ int Engine::addSharedResource(const char* name, const float* const* chans, size_
 void Engine::pruneSharedResources() {
     Lock lk(mu_);   // SharedResource.h:93-101: drop entries nobody else references
     dsync();
+    retireArrays({});   // the stream is drained: releases every retired array, the sample buffers voices stopped playing among them
     for (auto it = resources_.begin(); it != resources_.end();) {
         if (it->second.use_count() == 1) {
             if (it->second->dChannel0) dfree(it->second->dChannel0);
@@ -768,10 +788,9 @@ int Engine::createNode(Group& g, const Value& a1, const Value& a2) {   // Runtim
             n.props["channels"] = Value::number(1); n.props["size"] = Value::number(512);
             n.size = SCOPE_CHANNELS * SCOPE_RING; break;
         case NodeKind::Capture: n.size = bitceil((int) (size_t) sr_) + CAPTURE_SCRATCH; break;   // Capture.h:17
-        case NodeKind::Sample: {   // buffer pointer lo / hi, length + 1 (0: no buffer), startOffset, stopOffset: new rows are zero
-            int r = allocRows(g, 5, false, n.paramRow);
+        case NodeKind::Sample: {   // no buffer, offsets 0: new rows are zero
+            int r = allocRows(g, SAMPLE_PARAM_ROWS, false, n.paramRow);
             if (r != rc::Ok) return r;
-            n.voiceRes.assign((size_t) g.nv, nullptr);
         } break;
         case NodeKind::Fft: {   // wasm/FFT.h:18-26: ring of one channel, default size 1024 set through setProperty
             n.size = SCOPE_RING;
@@ -796,14 +815,30 @@ int Engine::appendChild(Group& g, const Value& a1, const Value& a2, const Value&
 
 int Engine::nodeSetProperty(Group& g, Node& n, const std::string& key, const Value& val, int vb, int ve) {
     // vb/ve are group-relative voice bounds; only per-voice capable props honour a sub-range.
+    const PerVoiceProp* pv = perVoiceProp(n.kind, key);
+    if (pv && pv->bits) {   // const.value (Core.h:142-152), rand.seed (Noise.h:13-23), sample.startOffset / stopOffset (Sample.h:56,69)
+        if (!val.isNumber()) return rc::InvalidPropertyType;
+        uint32_t bits;
+        if (!pv->bits(val.asNumber(), bits)) return rc::InvalidPropertyValue;
+        int r = fillRowBits(g, n.*pv->base + pv->row, vb, ve, bits);
+        if (r == rc::Ok && pv->shadow) r = fillRowBits(g, n.shadowRow, vb, ve, bits);
+        if (r != rc::Ok) return r;
+        n.props[key] = val;
+        return rc::Ok;
+    }
+    if (key == "seq" && isSeqFamily(n.kind)) {   // the whole group: a batch that sets `seq` cuts the group at its voice range first
+        std::vector<char> blob;
+        size_t count = 0;
+        int r = seqBlob(n.kind, val, blob, count);
+        if (r == rc::Ok) r = uploadArray(n.seqData, blob.data(), blob.size(), count);
+        if (r != rc::Ok) return r;
+        ++n.seqGen; g.codeDirty = true;
+        // the voices' own rows, if any, all take the new sequence
+        if (n.paramRow >= 0 && (r = assignVoiceArrays(g, n, {seqArray(n.seqData)}, nullptr, vb, ve, &n.seqGen)) != rc::Ok) return r;
+        n.props[key] = val;
+        return rc::Ok;
+    }
     switch (n.kind) {
-        case NodeKind::Const:
-            if (key == "value") {   // Core.h:142-152
-                if (!val.isNumber()) return rc::InvalidPropertyType;
-                int r = fillRow(g, n.paramRow, vb, ve, (float) val.asNumber());
-                if (r != rc::Ok) return r;
-            }
-            break;
         case NodeKind::Root:        // Core.h:33-64
             if (key == "active") {
                 if (!val.isBool()) return rc::InvalidPropertyType;
@@ -876,15 +911,6 @@ int Engine::nodeSetProperty(Group& g, Node& n, const std::string& key, const Val
                 n.holdSamples = static_cast<uint32_t>(h); g.codeDirty = true;
             }
             break;
-        case NodeKind::Rand:        // Noise.h:13-23
-            if (key == "seed") {
-                if (!val.isNumber()) return rc::InvalidPropertyType;
-                const uint32_t seed = static_cast<uint32_t>(val.asNumber());
-                int r = fillRowBits(g, n.stateRow, vb, ve, seed);
-                if (r == rc::Ok) r = fillRowBits(g, n.shadowRow, vb, ve, seed);
-                if (r != rc::Ok) return r;
-            }
-            break;
         case NodeKind::TapIn:
         case NodeKind::TapOut:      // Feedback.h:24-38,71-85
             if (key == "name") {
@@ -907,9 +933,7 @@ int Engine::nodeSetProperty(Group& g, Node& n, const std::string& key, const Val
                 if (!val.isString()) return rc::InvalidPropertyType;
                 auto it = resources_.find(val.asString());
                 if (it == resources_.end()) return rc::InvalidPropertyValue;
-                std::vector<std::shared_ptr<Resource>> res(1, it->second);
-                std::vector<int32_t> index((size_t) (ve - vb), 0);
-                int r = assignSampleBuffers(g, n, res, index.data(), vb, ve);
+                int r = assignSampleBuffers(g, n, {it->second}, nullptr, vb, ve);
                 if (r != rc::Ok) return r;
             }
             if (key == "mode") {
@@ -917,13 +941,6 @@ int Engine::nodeSetProperty(Group& g, Node& n, const std::string& key, const Val
                 const std::string& m = val.asString();
                 if (m == "trigger") n.mode = 0; if (m == "gate") n.mode = 1; if (m == "loop") n.mode = 2;
                 g.codeDirty = true;
-            }
-            if (key == "startOffset" || key == "stopOffset") {
-                if (!val.isNumber()) return rc::InvalidPropertyType;
-                const int v = static_cast<int>(val.asNumber());
-                if (v < 0) return rc::InvalidPropertyValue;
-                int r = fillRowBits(g, n.paramRow + (key == "startOffset" ? 3 : 4), vb, ve, (uint32_t) v);
-                if (r != rc::Ok) return r;
             }
             break;
 
@@ -946,7 +963,6 @@ int Engine::nodeSetProperty(Group& g, Node& n, const std::string& key, const Val
                 if (val.asNumber() < 0.0) return rc::InvalidPropertyValue;
                 n.seqOffset = static_cast<uint64_t>(val.asNumber()); g.codeDirty = true;
             }
-            if (key == "seq") { int r = setGroupSeq(g, n, val, vb, ve); if (r != rc::Ok) return r; }
             break;
         case NodeKind::SparSeq:     // SparSeq.h:40-124
             if (key == "offset") {
@@ -971,10 +987,8 @@ int Engine::nodeSetProperty(Group& g, Node& n, const std::string& key, const Val
                 if (val.asNumber() < 0.0) return rc::InvalidPropertyValue;
                 n.tickIntervalSamples = sr_ * val.asNumber(); g.codeDirty = true;
             }
-            if (key == "seq") { int r = setGroupSeq(g, n, val, vb, ve); if (r != rc::Ok) return r; }
             break;
         case NodeKind::SparSeq2:    // SparSeq2.h:20-56
-            if (key == "seq") { int r = setGroupSeq(g, n, val, vb, ve); if (r != rc::Ok) return r; }
             if (key == "interpolate") { if (!val.isNumber()) return rc::InvalidPropertyType; n.interpolate = static_cast<int32_t>(val.asNumber()); g.codeDirty = true; }
             break;
         case NodeKind::Scope:       // Analyzers.h:155-179
@@ -1087,8 +1101,8 @@ int Engine::applyToGroup(Group& g, const std::vector<Value>& batch, int vb, int 
 }
 
 bool Engine::isValueOnlyBatch(const std::vector<Value>& batch, int vb, int ve) {
-    // A batch made only of SET_PROPERTY on per-voice-capable props (const.value, rand.seed, once.arm, sample.startOffset / stopOffset) never changes the
-    // structure of a group, so it may address any sub-range of voices without splitting the group.
+    // A batch made only of SET_PROPERTY on per-voice-capable props (perVoiceProp) never changes the structure of a group, so it may
+    // address any sub-range of voices without splitting the group.
     for (auto& ins : batch) {
         if (!ins.isArray()) return false;
         auto& ar = ins.asArray();
@@ -1099,11 +1113,8 @@ bool Engine::isValueOnlyBatch(const std::vector<Value>& batch, int vb, int ve) {
             if (g->v0 >= ve || g->v0 + g->nv <= vb) continue;
             auto it = g->nodes.find(id);
             if (it == g->nodes.end()) return false;
-            const bool ok = (it->second.kind == NodeKind::Const && ar[2].asString() == "value" && ar[3].isNumber()) ||
-                            (it->second.kind == NodeKind::Rand && ar[2].asString() == "seed" && ar[3].isNumber()) ||
-                            (it->second.kind == NodeKind::Once && ar[2].asString() == "arm" && ar[3].isBool()) ||
-                            (it->second.kind == NodeKind::Sample && (ar[2].asString() == "startOffset" || ar[2].asString() == "stopOffset") && ar[3].isNumber());
-            if (!ok) return false;
+            const PerVoiceProp* p = perVoiceProp(it->second.kind, ar[2].asString());
+            if (!p || (p->bits ? !ar[3].isNumber() : !ar[3].isBool())) return false;
         }
     }
     return true;
@@ -1171,18 +1182,14 @@ int Engine::splitGroupsAt(int v) {
         for (auto& kv : g.nodes) {
             Node n = kv.second;   // host-side copy: props, inlets, fades, resource handles, row indices (same layout)
             n.ring = nullptr; n.tapPrivate = nullptr;
-            if (!kv.second.relay.empty()) {   // capture relay buffers follow their voices
-                n.relay.assign(kv.second.relay.begin() + std::min<size_t>(cut, kv.second.relay.size()), kv.second.relay.end());
-                kv.second.relay.resize(std::min<size_t>(cut, kv.second.relay.size()));
-            }
-            if (!kv.second.voiceRes.empty()) {   // so do the buffers sample voices play
-                n.voiceRes.assign(kv.second.voiceRes.begin() + std::min<size_t>(cut, kv.second.voiceRes.size()), kv.second.voiceRes.end());
-                kv.second.voiceRes.resize(std::min<size_t>(cut, kv.second.voiceRes.size()));
-            }
-            if (!kv.second.voiceSeq.empty()) {   // and the sequences seq-family voices read (their rows moved with the other rows)
-                n.voiceSeq.assign(kv.second.voiceSeq.begin() + std::min<size_t>(cut, kv.second.voiceSeq.size()), kv.second.voiceSeq.end());
-                kv.second.voiceSeq.resize(std::min<size_t>(cut, kv.second.voiceSeq.size()));
-            }
+            // per-voice host vectors follow their voices: capture relays, the arrays sample and seq-family voices read (rows moved above)
+            auto slice = [cut](auto& from, auto& to) {
+                const size_t c = std::min<size_t>(cut, from.size());
+                to.assign(from.begin() + c, from.end());
+                from.resize(c);
+            };
+            slice(kv.second.relay, n.relay);
+            slice(kv.second.voiceArrays, n.voiceArrays);
             if (kv.second.ring) {
                 if (!cloneTiles(kv.second.ring, (size_t) kv.second.size * L, &n.ring)) return rc::CudaError;
                 n.ringFloats = newTiles * (size_t) kv.second.size * L;
@@ -1305,24 +1312,41 @@ int Engine::applyBinary(int vb, int ve, const void* data, size_t bytes) {
     return applyBatch(vb, ve, batch);
 }
 
-int Engine::setConstTable(const int32_t* nodeIds, int nProps, const float* values, int vb, int count) {
-    Lock lk(mu_);
-    dsetdev();
-    if (vb < 0 || count < 0 || vb + count > numVoices_ || nProps < 0) return fail(rc::BadArgument, "voice range out of bounds");
+// The targets of a per-voice call, every check done before anything changes: the range, the node in every group, its kind.
+template <class KindOk>
+int Engine::voiceTargets(int32_t nodeId, int vb, int count, KindOk kindOk, const char* kindError, std::vector<VoiceTarget>& out) {
+    out.clear();
+    if (!voiceRangeOk(vb, count, numVoices_)) return fail(rc::BadArgument, "voice range out of bounds");
     for (auto& gp : groups_) {
         Group& g = *gp;
         const int b = std::max(vb, g.v0), e = std::min(vb + count, g.v0 + g.nv);
         if (b >= e) continue;
-        for (int p = 0; p < nProps; ++p) {
-            auto it = g.nodes.find(nodeIds[p]);
-            if (it == g.nodes.end()) return rc::NodeNotFound;
-            Node& n = it->second;
-            if (n.kind != NodeKind::Const) return fail(rc::InvalidPropertyType, "property table rows must address const nodes");
-            const float* src = values + (size_t) p * count + (b - vb);
-            if (!cuda(dmemcpy(g.dRows + (size_t) n.paramRow * g.Vpad + (b - g.v0), src, sizeof(float) * (size_t) (e - b), cudaMemcpyHostToDevice), "property table upload")) return rc::CudaError;
-            n.props["value"] = Value::number(src[e - b - 1]);
-        }
+        auto it = g.nodes.find(nodeId);
+        if (it == g.nodes.end()) { out.clear(); return fail(rc::NodeNotFound, "node not found"); }
+        if (!kindOk(it->second.kind)) { out.clear(); return fail(rc::InvalidPropertyType, kindError); }
+        out.push_back(VoiceTarget{g, it->second, b - g.v0, e - g.v0, b - vb});
     }
+    return rc::Ok;
+}
+
+int Engine::setConstTable(const int32_t* nodeIds, int nProps, const float* values, int vb, int count) {
+    Lock lk(mu_);
+    dsetdev();
+    if (nProps < 0 || !voiceRangeOk(vb, count, numVoices_)) return fail(rc::BadArgument, "voice range out of bounds");
+    // every check before any change: a failed call changes nothing
+    std::vector<std::vector<VoiceTarget>> targets((size_t) nProps);
+    for (int p = 0; p < nProps; ++p) {
+        const int r = voiceTargets(nodeIds[p], vb, count, [](NodeKind k) { return k == NodeKind::Const; },
+                                   "property table rows must address const nodes", targets[(size_t) p]);
+        if (r != rc::Ok) return r;
+    }
+    for (int p = 0; p < nProps; ++p)
+        for (auto& t : targets[(size_t) p]) {
+            const float* src = values + (size_t) p * count;
+            const int r = writeColumns(t.g, t.n.paramRow, 1, t.b, t.e - t.b, src + t.at, "property table upload");
+            if (r != rc::Ok) return r;
+            t.n.props["value"] = Value::number(src[t.last()]);
+        }
     return rc::Ok;
 }
 
@@ -1331,42 +1355,20 @@ int Engine::setPropertyPerVoice(int32_t nodeId, const char* key, const double* v
     // Vectorised SET_PROPERTY (SURVEY.md §8f N2): values[i] goes to voice vb+i. Same semantics as `count`
     // single-voice [3,id,key,value] batches, without `count` JSON parses.
     dsetdev();
-    if (vb < 0 || count < 0 || vb + count > numVoices_) return fail(rc::BadArgument, "voice range out of bounds");
     const std::string k(key);
-    const bool offsetKey = k == "startOffset" || k == "stopOffset";
     // every check before any change: a failed call changes nothing
-    for (auto& gp : groups_) {
-        const Group& g = *gp;
-        if (std::max(vb, g.v0) >= std::min(vb + count, g.v0 + g.nv)) continue;
-        auto it = g.nodes.find(nodeId);
-        if (it == g.nodes.end()) return rc::NodeNotFound;
-        const NodeKind kind = it->second.kind;
-        if (!((kind == NodeKind::Const && k == "value") || (kind == NodeKind::Rand && k == "seed") || (kind == NodeKind::Sample && offsetKey)))
-            return fail(rc::InvalidPropertyType, "property is not per-voice capable");
-    }
-    if (offsetKey)
-        for (int i = 0; i < count; ++i)
-            if (static_cast<int>(values[i]) < 0) return fail(rc::InvalidPropertyValue, "sample offsets must not be negative");   // Sample.h:56,69
-    for (auto& gp : groups_) {
-        Group& g = *gp;
-        const int b = std::max(vb, g.v0), e = std::min(vb + count, g.v0 + g.nv);
-        if (b >= e) continue;
-        Node& n = g.nodes.find(nodeId)->second;
-        int row, shadow = -1;
-        std::vector<uint32_t> bits((size_t) (e - b));
-        if (n.kind == NodeKind::Const && k == "value") {
-            row = n.paramRow;
-            for (int v = b; v < e; ++v) { float f = (float) values[v - vb]; std::memcpy(&bits[v - b], &f, 4); }
-        } else if (n.kind == NodeKind::Rand && k == "seed") {
-            row = n.stateRow; shadow = n.shadowRow;
-            for (int v = b; v < e; ++v) bits[v - b] = static_cast<uint32_t>(values[v - vb]);
-        } else {   // sample startOffset / stopOffset
-            row = n.paramRow + (k == "startOffset" ? 3 : 4);
-            for (int v = b; v < e; ++v) bits[v - b] = (uint32_t) static_cast<int>(values[v - vb]);
-        }
-        for (int r : {row, shadow})   // pageable source: staged before the call returns
-            if (r >= 0 && !cuda(dmemcpy(g.dRows + (size_t) r * g.Vpad + (b - g.v0), bits.data(), sizeof(uint32_t) * bits.size(), cudaMemcpyHostToDevice), "per-voice prop upload")) return rc::CudaError;
-        n.props[k] = Value::number(values[e - 1 - vb]);
+    std::vector<VoiceTarget> targets;
+    int r = voiceTargets(nodeId, vb, count, [&](NodeKind kind) { const PerVoiceProp* p = perVoiceProp(kind, k); return p && p->bits; },
+                         "property is not per-voice capable", targets);
+    if (r != rc::Ok || targets.empty()) return r;
+    const PerVoiceProp& prop = *perVoiceProp(targets[0].n.kind, k);   // the key names one kind
+    std::vector<uint32_t> bits((size_t) count);
+    for (int i = 0; i < count; ++i)
+        if (!prop.bits(values[i], bits[(size_t) i])) return fail(rc::InvalidPropertyValue, "sample offsets must not be negative");
+    for (auto& t : targets) {
+        for (int row : {t.n.*prop.base + prop.row, prop.shadow ? t.n.shadowRow : -1})
+            if (row >= 0 && (r = writeColumns(t.g, row, 1, t.b, t.e - t.b, bits.data() + t.at, "per-voice prop upload")) != rc::Ok) return r;
+        t.n.props[k] = Value::number(values[t.last()]);
     }
     return rc::Ok;
 }
@@ -1374,17 +1376,14 @@ int Engine::setPropertyPerVoice(int32_t nodeId, const char* key, const double* v
 int Engine::setPathPerVoice(int32_t nodeId, const char* const* names, int numNames, const int32_t* index, int vb, int count) {
     Lock lk(mu_);
     dsetdev();
-    if (vb < 0 || count < 0 || vb + count > numVoices_ || numNames < 0) return fail(rc::BadArgument, "voice range out of bounds");
+    if (numNames < 0) return fail(rc::BadArgument, "voice range out of bounds");
     for (int i = 0; i < count; ++i)
         if (index[i] < 0 || index[i] >= numNames) return fail(rc::BadArgument, "name index out of range");
     // every check before any change: a failed call changes nothing
-    for (auto& gp : groups_) {
-        const Group& g = *gp;
-        if (std::max(vb, g.v0) >= std::min(vb + count, g.v0 + g.nv)) continue;
-        auto it = g.nodes.find(nodeId);
-        if (it == g.nodes.end()) return rc::NodeNotFound;
-        if (it->second.kind != NodeKind::Convolve && it->second.kind != NodeKind::Sample) return fail(rc::InvalidPropertyType, "property is not per-voice capable");
-    }
+    std::vector<VoiceTarget> targets;
+    const int rt = voiceTargets(nodeId, vb, count, [](NodeKind k) { return k == NodeKind::Convolve || k == NodeKind::Sample; },
+                                "property is not per-voice capable", targets);
+    if (rt != rc::Ok) return rt;
     std::vector<std::shared_ptr<Resource>> res((size_t) numNames);
     for (int k = 0; k < numNames; ++k) {
         auto it = names[k] ? resources_.find(names[k]) : resources_.end();
@@ -1403,15 +1402,14 @@ int Engine::setPathPerVoice(int32_t nodeId, const char* const* names, int numNam
         }
         return spectra[(size_t) k];
     };
-    for (auto& gp : groups_) {
-        Group& g = *gp;
-        const int b = std::max(vb, g.v0), e = std::min(vb + count, g.v0 + g.nv);
-        if (b >= e) continue;
-        Node& n = g.nodes.find(nodeId)->second;
+    for (auto& t : targets) {
+        Group& g = t.g;
+        Node& n = t.n;
+        const int last = index[t.last()];
         if (n.kind == NodeKind::Sample) {
-            const int r = assignSampleBuffers(g, n, res, index + (b - vb), b - g.v0, e - g.v0);
+            const int r = assignSampleBuffers(g, n, res, index + t.at, t.b, t.e);
             if (r != rc::Ok) return r;
-            n.props["path"] = Value::string(names[index[e - 1 - vb]]);
+            n.props["path"] = Value::string(names[last]);
             continue;
         }
         std::string err;
@@ -1425,11 +1423,10 @@ int Engine::setPathPerVoice(int32_t nodeId, const char* const* names, int numNam
             n.conv = cs;
             n.resourceDirty = false;
         }
-        std::vector<std::shared_ptr<IrSpectra>> h((size_t) (e - b));
-        for (int v = b; v < e; ++v)
-            if (!(h[(size_t) (v - b)] = spectraOf(index[v - vb], err))) return fail(rc::CudaError, err);
-        if (!convolver_assign(*n.conv, b - g.v0, e - b, h, stream_, err)) return fail(rc::CudaError, err);
-        const int last = index[e - 1 - vb];   // snapshot(): the value last set for the group's highest addressed voice
+        std::vector<std::shared_ptr<IrSpectra>> h((size_t) (t.e - t.b));
+        for (int i = 0; i < t.e - t.b; ++i)
+            if (!(h[(size_t) i] = spectraOf(index[t.at + i], err))) return fail(rc::CudaError, err);
+        if (!convolver_assign(*n.conv, t.b, t.e - t.b, h, stream_, err)) return fail(rc::CudaError, err);
         n.resource = res[(size_t) last];
         n.props["path"] = Value::string(names[last]);
         if (!hadResource) g.codeDirty = true;   // the program emitted silence for a convolver without an IR
@@ -1589,12 +1586,12 @@ int Engine::gc(int voice, std::vector<int32_t>& pruned) {
 
 void Engine::reset() {
     Lock lk(mu_);
-    // Runtime.h:449-458: only SampleNode does anything on reset(): noteOff on both readers (targetGain rows 4 and 6)
+    // Runtime.h:449-458: only SampleNode does anything on reset(): noteOff on both readers (their target gains)
     dsetdev();
     for (auto& gp : groups_)
         for (auto& kv : gp->nodes)
             if (kv.second.kind == NodeKind::Sample)
-                for (int k : {4, 6}) fillRowBits(*gp, kv.second.stateRow + k, 0, gp->nv, 0u);
+                for (int k : {SAMPLE_TARGET_GAIN0, SAMPLE_TARGET_GAIN1}) fillRowBits(*gp, kv.second.stateRow + k, 0, gp->nv, 0u);
 }
 
 // Voice vb + i (group-relative, i < ve - vb) of sample node n plays res[index[i]] from the next block on with fresh readers
@@ -1602,24 +1599,19 @@ void Engine::reset() {
 int Engine::assignSampleBuffers(Group& g, Node& n, const std::vector<std::shared_ptr<Resource>>& res, const int32_t* index, int vb, int ve) {
     const int cnt = ve - vb;
     if (cnt <= 0) return rc::Ok;
-    for (auto& r : res) { const int e = ensureResourceOnDevice(*r); if (e != rc::Ok) return e; }
-    std::vector<uint32_t> desc((size_t) 3 * cnt);
-    for (int i = 0; i < cnt; ++i) {
-        const Resource& r = *res[(size_t) index[i]];
-        const uint64_t p = (uint64_t) (uintptr_t) r.dChannel0;
-        desc[(size_t) i] = (uint32_t) p;
-        desc[(size_t) cnt + i] = (uint32_t) (p >> 32);
-        desc[(size_t) 2 * cnt + i] = (uint32_t) r.numSamples + 1u;
+    std::vector<VoiceArray> arrs;
+    for (auto& r : res) {
+        const int e = ensureResourceOnDevice(*r);
+        if (e != rc::Ok) return e;
+        arrs.push_back(VoiceArray{r, (uint64_t) (uintptr_t) r->dChannel0, (uint32_t) r->numSamples + 1u});
     }
-    for (int k = 0; k < 3; ++k)   // pageable source: staged before the call returns
-        if (!cuda(dmemcpy(g.dRows + (size_t) (n.paramRow + k) * g.Vpad + vb, desc.data() + (size_t) k * cnt, sizeof(uint32_t) * cnt, cudaMemcpyHostToDevice), "sample buffer rows")) return rc::CudaError;
-    // reader state: two double rows (the positions, 2 * vb ..) then the four gain rows
-    if (!cuda(dmemset(g.dRows + (size_t) n.stateRow * g.Vpad + 2 * (size_t) vb, 0, sizeof(double) * cnt), "sample reader reset")) return rc::CudaError;
-    if (!cuda(dmemset(g.dRows + (size_t) (n.stateRow + 2) * g.Vpad + 2 * (size_t) vb, 0, sizeof(double) * cnt), "sample reader reset")) return rc::CudaError;
-    for (int k = 4; k < 8; ++k) { const int e = fillRowBits(g, n.stateRow + k, vb, ve, 0u); if (e != rc::Ok) return e; }
-    if (n.voiceRes.size() < (size_t) g.nv) n.voiceRes.resize((size_t) g.nv);
-    for (int i = 0; i < cnt; ++i) n.voiceRes[(size_t) (vb + i)] = res[(size_t) index[i]];
-    steadyValid_ = false;
+    int e = assignVoiceArrays(g, n, arrs, index, vb, ve);
+    if (e != rc::Ok) return e;
+    // the readers: positions are double rows (2 * vb ..), then the gain rows
+    for (int k : {SAMPLE_POS0, SAMPLE_POS1})
+        if (!cuda(dmemset(g.dRows + (size_t) (n.stateRow + k) * g.Vpad + 2 * (size_t) vb, 0, sizeof(double) * cnt), "sample reader reset")) return rc::CudaError;
+    for (int k = SAMPLE_TARGET_GAIN0; k < SAMPLE_GAINS_END; ++k)
+        if ((e = fillRowBits(g, n.stateRow + k, vb, ve, 0u)) != rc::Ok) return e;
     return rc::Ok;
 }
 
@@ -1788,7 +1780,7 @@ int Compiler::emitNode(Node& n, int rootIndex) {
     // The seq family reads the group's sequence (ptr = data, aux0 = count), or after setSeqPerVoice each voice's own: mode bit 3 and four
     // parameter rows after the inputs (data pointer low / high word, count, generation).  A voice without a sequence reads count 0.
     auto seqSource = [&]() {
-        if (n.paramRow >= 0) { op.mode |= 8u; for (int k = 0; k < 4; ++k) op.operands.push_back({K_PARAM, n.paramRow + k}); }
+        if (n.paramRow >= 0) { op.mode |= 8u; for (int k = 0; k < SEQ_PARAM_ROWS; ++k) op.operands.push_back({K_PARAM, n.paramRow + k}); }
         else if (n.seqData) { op.aux0 = (uint32_t) n.seqData->count; op.ptr = (uint64_t) (uintptr_t) n.seqData->d; prog.pinned.push_back(n.seqData); }
     };
 
@@ -1950,7 +1942,7 @@ int Compiler::emitNode(Node& n, int rootIndex) {
             op.mode = (uint32_t) n.mode | (numCh >= 2 ? 4u : 0u);
             // VariablePitchLerpReader(float sampleRate, ...): 1 - exp(-1 / (0.01 * sampleRate)) in double, stored as float
             op.aux0 = fbits((float) (1.0 - std::exp(-1.0 / (0.01 * (double) (float) E.sr_))));
-            for (int k = 0; k < 5; ++k) op.operands.push_back({K_PARAM, n.paramRow + k});
+            for (int k = 0; k < SAMPLE_PARAM_ROWS; ++k) op.operands.push_back({K_PARAM, n.paramRow + k});
         } break;
 
         case NodeKind::TapIn:

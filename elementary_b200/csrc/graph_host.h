@@ -47,6 +47,7 @@ struct DeviceArray {
     bool planOnly = false;
     ~DeviceArray();
 };
+struct VoiceArray; struct VoiceTarget;   // graph_host.cpp: the per-voice setters
 
 struct Inlet { int32_t source; int32_t channel; };
 
@@ -83,8 +84,7 @@ struct Node {
     std::vector<Inlet> inlets;
     std::map<std::string, Value> props;
 
-    int paramRow = -1;               // const / sr: per-voice parameter row; sample: the first of five (ctl_sample, render_kernel.cu);
-                                     // seq family: the first of four, made by the first setSeqPerVoice (ctl_seq_src, render_kernel.cu)
+    int paramRow = -1;               // const / sr: per-voice parameter row; sample, seq family (from its first setSeqPerVoice): the first of its rows
     int stateRow = -1;               // first scalar state row (even-aligned when it holds doubles)
     int shadowRow = -1;              // rand / once: the seed / arm last set for each voice, outside the state rows (resetVoices)
     int mode = 0;                    // svf / svfshelf / mm1p / sample mode
@@ -99,12 +99,11 @@ struct Node {
     std::string tapName;
     float* tapPrivate = nullptr;     // tapOut private delayBuffer
     std::shared_ptr<Resource> resource;   // table / convolve
-    std::vector<std::shared_ptr<Resource>> voiceRes;   // sample: the buffer each voice of the group plays (kept alive while it does)
+    std::vector<std::shared_ptr<const void>> voiceArrays;   // sample / seq family with paramRow >= 0: keeps each voice's buffer (Resource) or sequence (DeviceArray) alive
     bool resourceDirty = false;
     std::shared_ptr<ConvolverState> conv;
     // seq / seq2 / sparseq / sparseq2 (Core.h:411-466, Seq2.h:39-84, SparSeq.h:40-124, SparSeq2.h:20-56)
     std::shared_ptr<DeviceArray> seqData;
-    std::vector<std::shared_ptr<DeviceArray>> voiceSeq;   // with paramRow >= 0: the sequence each voice of the group reads
     uint32_t seqGen = 0, loopGen = 0;
     bool seqHold = false, seqLoop = true, follow = false;
     uint64_t seqOffset = 0;
@@ -483,6 +482,7 @@ private:
     int createNode(Group& g, const Value& id, const Value& type);
     int appendChild(Group& g, const Value& parent, const Value& child, const Value& chan);
     int setProperty(Group& g, const Value& id, const Value& key, const Value& val, int vb, int ve);
+    template <class KindOk> int voiceTargets(int32_t nodeId, int vb, int count, KindOk kindOk, const char* kindError, std::vector<VoiceTarget>& out);
     int activateRoots(Group& g, const Value& roots);
     int nodeSetProperty(Group& g, Node& n, const std::string& key, const Value& val, int vb, int ve);
     bool isValueOnlyBatch(const std::vector<Value>& batch, int vb, int ve);
@@ -496,14 +496,13 @@ private:
     int fillRow(Group& g, int row, int vb, int ve, float value);
     int fillRowBits(Group& g, int row, int vb, int ve, uint32_t bits);
     int ensureResourceOnDevice(Resource& r);
+    int writeColumns(Group& g, int row, int rows, int vb, int cnt, const void* words, const char* what);
+    int assignVoiceArrays(Group& g, Node& n, const std::vector<VoiceArray>& arrs, const int32_t* index, int vb, int ve, const uint32_t* gen = nullptr);
     int assignSampleBuffers(Group& g, Node& n, const std::vector<std::shared_ptr<Resource>>& res, const int32_t* index, int vb, int ve);
     int uploadArray(std::shared_ptr<DeviceArray>& out, const void* data, size_t bytes, size_t count);
-    int setGroupSeq(Group& g, Node& n, const Value& val, int vb, int ve);
-    int ensureSeqRows(Group& g, Node& n);
-    int assignSeqRows(Group& g, Node& n, const std::vector<std::shared_ptr<DeviceArray>>& arrs, const int32_t* index, int vb, int ve);
-    void retireArrays(std::vector<std::shared_ptr<DeviceArray>>&& arrs);
-    // sequence arrays no voice reads any more, each batch released once the stream has passed its event (retireArrays)
-    std::deque<std::pair<cudaEvent_t, std::vector<std::shared_ptr<DeviceArray>>>> retiredArrays_;
+    void retireArrays(std::vector<std::shared_ptr<const void>>&& arrs);
+    // arrays no voice reads any more (voiceArrays), each batch released once the stream has passed its event (retireArrays)
+    std::deque<std::pair<cudaEvent_t, std::vector<std::shared_ptr<const void>>>> retiredArrays_;
 
     // compile (Runtime.h:521-577 + GraphRenderSequence.h:107-187)
     int compile(Group& g, int nIn, std::shared_ptr<Program>& out);

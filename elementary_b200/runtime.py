@@ -221,22 +221,22 @@ class Runtime:
         """Voice ``voice_begin + i`` of convolve or sample node ``node_id`` gets the impulse response or sample buffer
         ``names[index[i]]`` (shared resources), without cutting its voice group; the addressed voices restart from silence at the next
         block (a sample node keeps its voices' trigger edge detector and current reader)."""
-        enc = [n.encode() if isinstance(n, str) else bytes(n) for n in names]
-        tab = (C.c_char_p * max(1, len(enc)))(*enc)
-        idx = np.ascontiguousarray(np.asarray(index, dtype=np.int32).reshape(-1))
-        return self._lib.elem_b200_set_path_per_voice(self._h, int(node_id), tab, len(enc),
-                                                      idx.ctypes.data_as(C.POINTER(C.c_int32)), int(voice_begin), idx.size)
+        return self._set_per_voice(self._lib.elem_b200_set_path_per_voice, node_id,
+                                   [n.encode() if isinstance(n, str) else bytes(n) for n in names], index, voice_begin)
 
     def set_seq_per_voice(self, node_id: int, seqs, index, voice_begin: int = 0) -> int:
         """Voice ``voice_begin + i`` of seq, seq2, sparseq or sparseq2 node ``node_id`` gets the sequence ``seqs[index[i]]`` (a Python
         value such as ``[1, 2, 3]`` or ``[{"tickTime": 0, "value": 1}]``, JSON-encoded here; bytes pass through as JSON text),
         without cutting its voice group: the same as single-voice ``[3, node_id, "seq", seqs[index[i]]]`` batches.  Each distinct
         sequence is parsed and uploaded once."""
-        enc = [s if isinstance(s, bytes) else json.dumps(s).encode() for s in seqs]
-        tab = (C.c_char_p * max(1, len(enc)))(*enc)
+        return self._set_per_voice(self._lib.elem_b200_set_seq_per_voice, node_id,
+                                   [s if isinstance(s, bytes) else json.dumps(s).encode() for s in seqs], index, voice_begin)
+
+    def _set_per_voice(self, fn, node_id, table, index, voice_begin):
+        """fn(node, table of C strings, their count, int32 index per voice, first voice, voice count): a table plus an index."""
+        tab = (C.c_char_p * max(1, len(table)))(*table)
         idx = np.ascontiguousarray(np.asarray(index, dtype=np.int32).reshape(-1))
-        return self._lib.elem_b200_set_seq_per_voice(self._h, int(node_id), tab, len(enc),
-                                                     idx.ctypes.data_as(C.POINTER(C.c_int32)), int(voice_begin), idx.size)
+        return fn(self._h, int(node_id), tab, len(table), idx.ctypes.data_as(C.POINTER(C.c_int32)), int(voice_begin), idx.size)
 
     def reset_voices(self, voices) -> int:
         """The given voices (runtime-global indices, any order, repeats allowed) restart as fresh instances from the next block on, as

@@ -59,7 +59,10 @@ int elem_b200_apply_binary(elem_b200_runtime* rt, int voiceBegin, int voiceEnd, 
 
 /* Per-voice property TABLE: values[p][i] (float32, row-major, numProps rows of `count`) -> the `value` prop of const node nodeIds[p]
  * for voice voiceBegin+i.  One device copy per row straight from the caller's table: a million voices x a dozen per-voice constants
- * are a dozen copies, not a dozen million JSON numbers.  Equivalent to the [[3,nodeIds[p],"value",values[p][i]]] batches. */
+ * are a dozen copies, not a dozen million JSON numbers.  Equivalent to the [[3,nodeIds[p],"value",values[p][i]]] batches.
+ * Returns -2 for a voice range out of bounds or a negative numProps, NodeNotFound (2) when a voice group in the range lacks one of
+ * the nodes, InvalidPropertyType (5) when one is not a const.  All of it is checked before anything changes: a failed call changes
+ * nothing. */
 int elem_b200_set_const_table(elem_b200_runtime* rt, const int32_t* nodeIds, int numProps, const float* values, int voiceBegin, int count);
 
 /* Vectorised SET_PROPERTY: values[i] -> voice voiceBegin+i; equivalent to `count` single-voice
