@@ -121,6 +121,15 @@ int elem_b200_process_offline_events(elem_b200_runtime* rt, const float* const* 
                                            voiceBegin, voiceEnd, cb, user));
 }
 
+int elem_b200_process_offline_readouts(elem_b200_runtime* rt, const float* const* in, size_t nIn, const float* inVoices,
+                                       float* const* mixOut, float* voicesOut, size_t nOut, size_t numSamples,
+                                       size_t chunkBlocks, void* userData,
+                                       const int32_t* nodeIds, int numNodes, int voiceBegin, int count,
+                                       float* a, float* b, uint8_t* fresh) {
+    GUARD(rt->engine->processOfflineReadouts(in, nIn, inVoices, mixOut, voicesOut, nOut, numSamples, chunkBlocks, static_cast<const int64_t*>(userData),
+                                             nodeIds, numNodes, voiceBegin, count, a, b, fresh));
+}
+
 int elem_b200_enqueue_block(elem_b200_runtime* rt, size_t nIn, size_t nOut, size_t numSamples, int flags) {
     GUARD(rt->engine->enqueueBlock(nIn, nOut, numSamples, (flags & 1) != 0, (flags & 2) != 0, (flags & 4) != 0, (flags & 8) != 0));
 }
@@ -189,6 +198,20 @@ int elem_b200_process_queued_events_range(elem_b200_runtime* rt, int voiceBegin,
 
 void elem_b200_process_queued_events(elem_b200_runtime* rt, elem_b200_event_cb cb, void* user) {
     (void) elem_b200_process_queued_events_range(rt, 0, -1, cb, user);
+}
+
+int elem_b200_poll_readouts(elem_b200_runtime* rt, int32_t nodeId, int voiceBegin, int count, float* a, float* b, uint8_t* fresh, int flags) {
+    GUARD(rt->engine->pollReadouts(nodeId, voiceBegin, count, a, b, fresh, (flags & ELEM_B200_READOUT_DEVICE) != 0));
+}
+
+int elem_b200_node_type(elem_b200_runtime* rt, int voice, int32_t nodeId, char* buf, size_t cap) {
+    if (!rt) return 0;
+    try {
+        const std::string s = rt->engine->nodeType(voice, nodeId);
+        if (s.empty()) return 0;
+        if (buf && cap) { const size_t k = s.size() < cap - 1 ? s.size() : cap - 1; std::memcpy(buf, s.data(), k); buf[k] = 0; }
+        return (int) s.size() + 1;
+    } catch (...) { return 0; }
 }
 
 int elem_b200_set_option(elem_b200_runtime* rt, const char* key, double value) {

@@ -7,12 +7,33 @@
 // the next block sees the state a process() + processQueuedEvents() loop leaves behind.  Scope / fft windows are only read: their read
 // positions are the same for every voice of a group and live on the host.
 //
-// grid.y = item; grid.x strides over the item's work: a voice per thread (rows), a voice per warp (capture), a float per thread (window).
+// The same kernel serves the array poll (Engine::pollReadouts, EVLOG_READOUT items): meter / snapshot readouts written straight into
+// caller arrays, with the live poll's side effect.
+//
+// grid.y = item; grid.x strides over the item's work: a voice per thread (rows, readouts), a voice per warp (capture), a float per
+// thread (window).
 #include <algorithm>
 
 #include "kernels.h"
 
 namespace eb {
+
+// EVLOG_READOUT (kernels.h); out of line, so that the other item kinds keep their register allocation
+__device__ __noinline__ void readout_item(const EventLogItem& it, long long tid, long long nth) {
+    for (long long i = tid; i < it.n; i += nth) {
+        uint8_t f = 0;
+        if (it.drain) {
+            uint32_t* row = it.rows + it.b + i;
+            f = row[2 * it.Vpad] % 32u != 0u;     // the 32-slot queue arithmetic of the live poll (events_host.cpp emitPoll)
+            if (f) {
+                it.outA[i] = row[it.aRow * it.Vpad];
+                if (it.outB) it.outB[i] = row[it.Vpad];
+            }
+            row[2 * it.Vpad] = 0u;
+        }
+        it.fresh[i] = f;
+    }
+}
 
 __global__ void __launch_bounds__(256) event_log_kernel(const __grid_constant__ EventLogBatch batch) {
     const EventLogItem& it = batch.item[blockIdx.y];
@@ -45,6 +66,8 @@ __global__ void __launch_bounds__(256) event_log_kernel(const __grid_constant__ 
                 it.rows[4 * (size_t) it.Vpad + v] = 0u;
             }
         }
+    } else if (it.kind == EVLOG_READOUT) {
+        readout_item(it, tid, nth);
     } else {
         const long long per = (long long) it.size * it.L, total = (long long) (it.t1 - it.t0) * it.nch * per;
         float* const dst = reinterpret_cast<float*>(it.log);
@@ -62,7 +85,7 @@ cudaError_t launch_event_log(const EventLogBatch& batch, cudaStream_t stream) {
     long long work = 1;
     for (int k = 0; k < batch.n; ++k) {
         const EventLogItem& it = batch.item[k];
-        const long long w = it.kind == EVLOG_ROWS ? it.n : it.kind == EVLOG_CAPTURE ? 32LL * it.n
+        const long long w = (it.kind == EVLOG_ROWS || it.kind == EVLOG_READOUT) ? it.n : it.kind == EVLOG_CAPTURE ? 32LL * it.n
                                                                                       : (long long) (it.t1 - it.t0) * it.nch * it.size * it.L;
         work = w > work ? w : work;
     }

@@ -7,6 +7,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <set>
 #include <string>
 #include <vector>
 
@@ -452,13 +453,7 @@ int Engine::eventLogBlock(EventLog& log, int slot, size_t inChunk) {
     uint32_t* const base = reinterpret_cast<uint32_t*>(offLog_.dev[slot]);
     EventLogBatch batch;
     batch.n = 0;
-    auto flush = [&]() -> bool {
-        if (batch.n == 0) return true;
-        if (!cuda(launch_event_log(batch, stream_), "event log kernel launch")) return false;
-        ++launches_;
-        batch.n = 0;
-        return true;
-    };
+    auto flush = [&]() -> bool { return flushEventLog(batch) == rc::Ok; };
     for (PollItem& it : items) {
         it.logOff = log.used[slot];
         const size_t words = pollRecordWords(it);
@@ -486,6 +481,15 @@ int Engine::eventLogBlock(EventLog& log, int slot, size_t inChunk) {
     return flush() ? rc::Ok : rc::CudaError;
 }
 
+// One K5 launch of the items gathered in `batch`, which is emptied.
+int Engine::flushEventLog(EventLogBatch& batch) {
+    if (batch.n == 0) return rc::Ok;
+    if (!cuda(launch_event_log(batch, stream_), "event log kernel launch")) return rc::CudaError;
+    ++launches_;
+    batch.n = 0;
+    return rc::Ok;
+}
+
 // After the chunk in `slot` was scattered (its log is in pinned memory): its blocks' events, in block order, through the live formatter.
 int Engine::eventLogReplay(EventLog& log, int slot, size_t firstBlock) {
     LogSource src(*this, reinterpret_cast<const uint32_t*>(offLog_.pinned[slot]), (uint32_t) (blockSize_ + CAPTURE_SCRATCH));
@@ -502,6 +506,106 @@ int Engine::eventLogReplay(EventLog& log, int slot, size_t firstBlock) {
         ++relay.block;
     }
     return rc::Ok;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Array polls: the readouts of one meter / snapshot node for a range of voices, written by K5 (EVLOG_READOUT) into dense arrays instead
+// of one JSON event per voice.  The rules are those of processQueuedEvents: the voice groups where that poll reaches the node (the
+// sequence process() last used, an active root; forEachPolled) report and drain their queues, the others report nothing and keep them.
+
+// The (group, node) pairs a poll of voices [vb, ve) reaches: one walk, shared by every node a call or an offline block polls.
+int Engine::readoutPolled(int vb, int ve, PolledSet& out) {
+    out.clear();
+    return forEachPolled(vb, ve, false, [&](Group& g, Node& n, int, int) -> int {
+        out.insert({&g, n.id});
+        return rc::Ok;
+    });
+}
+
+int Engine::readoutEnqueue(int32_t nodeId, const std::vector<VoiceTarget>& targets, const PolledSet& polled, uint32_t* a, uint32_t* b,
+                           uint8_t* fresh, EventLogBatch& batch) {
+    for (const VoiceTarget& t : targets) {
+        EventLogItem& d = batch.item[batch.n++];
+        d = EventLogItem{};
+        d.kind = EVLOG_READOUT;
+        d.b = t.b; d.n = t.e - t.b; d.Vpad = t.g.Vpad; d.L = t.g.tileWidth;
+        d.drain = polled.count({&t.g, nodeId}) ? 1 : 0;
+        if (d.drain) d.rows = reinterpret_cast<uint32_t*>(t.g.dRows + (size_t) t.n.stateRow * t.g.Vpad);
+        d.aRow = t.n.kind == NodeKind::Meter ? 0 : 1;   // meter: rows min, max; snapshot: row 1 is the latched value (emitPoll)
+        d.outA = a + t.at;
+        d.outB = (b && t.n.kind == NodeKind::Meter) ? b + t.at : nullptr;
+        d.fresh = fresh + t.at;
+        if (batch.n == EVENT_LOG_BATCH) {
+            const int r = flushEventLog(batch);
+            if (r != rc::Ok) return r;
+        }
+    }
+    return rc::Ok;
+}
+
+// A record of readoutWords(count) words (a, b, fresh bytes) into the caller's arrays: fresh everywhere, a and b where fresh.  b is null
+// for a snapshot, whose record carries no b (the caller's b is never written).
+static void readoutCopy(const uint32_t* rec, int count, float* a, float* b, uint8_t* fresh) {
+    const uint8_t* f = reinterpret_cast<const uint8_t*>(rec + 2 * (size_t) count);
+    for (int i = 0; i < count; ++i) {
+        fresh[i] = f[i];
+        if (!f[i]) continue;
+        std::memcpy(a + i, rec + i, 4);
+        if (b) std::memcpy(b + i, rec + count + i, 4);
+    }
+}
+
+int Engine::pollReadouts(int32_t nodeId, int vb, int count, float* a, float* b, uint8_t* fresh, bool device) {
+    Lock lk(mu_);
+    if (count > 0 && (!a || !fresh)) return fail(rc::BadArgument, "pollReadouts: a or fresh is NULL");
+    std::vector<VoiceTarget> targets;
+    int r = readoutTargets(nodeId, vb, count, targets);
+    if (r != rc::Ok || count == 0) return r;
+    if (planOnly_) return fail(rc::CudaError, "plan-only runtime (no CUDA device): there are no readouts to poll");
+    dsetdev();
+    PolledSet polled;
+    if ((r = readoutPolled(vb, vb + count, polled)) != rc::Ok) return r;
+    EventLogBatch batch;
+    batch.n = 0;
+    if (device) {
+        if ((r = readoutEnqueue(nodeId, targets, polled, reinterpret_cast<uint32_t*>(a), reinterpret_cast<uint32_t*>(b), fresh, batch)) != rc::Ok) return r;
+        return flushEventLog(batch);
+    }
+    // host arrays: K5 fills a device staging record, which comes down in one copy
+    const size_t words = readoutWords(count);
+    if (!grow(dReadout_, readoutCap_, words, "cudaMalloc readout staging") ||
+        !grow(hReadout_, readoutPinned_, words, "cudaMallocHost readout staging", false, 1, true)) return rc::CudaError;
+    if ((r = readoutEnqueue(nodeId, targets, polled, dReadout_, dReadout_ + count, reinterpret_cast<uint8_t*>(dReadout_ + 2 * (size_t) count), batch)) != rc::Ok ||
+        (r = flushEventLog(batch)) != rc::Ok) return r;
+    if (!cuda(cudaMemcpyAsync(hReadout_, dReadout_, words * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream_), "D2H readouts") ||
+        !cuda(cudaStreamSynchronize(stream_), "sync after readouts")) return rc::CudaError;
+    readoutCopy(hReadout_, count, a, targets.front().n.kind == NodeKind::Meter ? b : nullptr, fresh);
+    return rc::Ok;
+}
+
+// After block inChunk of the chunk in `slot` was enqueued: every listed node's poll into the block's records in the chunk's log.
+int Engine::readoutBlock(ReadoutLog& ro, int slot, size_t inChunk) {
+    const size_t w = readoutWords(ro.count);
+    uint32_t* const rec = reinterpret_cast<uint32_t*>(offLog_.dev[slot]) + inChunk * ro.blockWords();
+    int r = readoutPolled(ro.vb, ro.vb + ro.count, ro.polled);     // the active program may change at any block: one walk per block
+    if (r != rc::Ok) return r;
+    EventLogBatch batch;
+    batch.n = 0;
+    for (size_t j = 0; j < ro.nodes.size(); ++j) {
+        uint32_t* const base = rec + j * w;
+        r = readoutEnqueue(ro.nodes[j], ro.targets[j], ro.polled, base, base + ro.count, reinterpret_cast<uint8_t*>(base + 2 * (size_t) ro.count), batch);
+        if (r != rc::Ok) return r;
+    }
+    return flushEventLog(batch);
+}
+
+void Engine::readoutScatter(const ReadoutLog& ro, const uint32_t* rec, size_t block) {
+    const size_t w = readoutWords(ro.count);
+    for (size_t j = 0; j < ro.nodes.size(); ++j) {
+        const size_t at = (j * ro.numBlocks + block) * (size_t) ro.count;
+        const bool meter = ro.targets[j].front().n.kind == NodeKind::Meter;   // every group has the same kind (readoutTargets)
+        readoutCopy(rec + j * w, ro.count, ro.a + at, ro.b && meter ? ro.b + at : nullptr, ro.fresh + at);
+    }
 }
 
 } // namespace eb

@@ -87,6 +87,7 @@ template <typename T> bool Engine::grow(T*& p, size_t& cap, size_t n, const char
     cap = n * slack;
     return true;
 }
+template bool Engine::grow<uint32_t>(uint32_t*&, size_t&, size_t, const char*, bool, size_t, bool);   // events_host.cpp: readout staging
 void Engine::dsync() { if (!planOnly_ && stream_) cudaStreamSynchronize(stream_); }
 void Engine::dsetdev() { if (!planOnly_) cudaSetDevice(device_); }
 void Engine::setStream(cudaStream_t s) {
@@ -168,7 +169,6 @@ constexpr int SAMPLE_POS0 = 0, SAMPLE_POS1 = 2, SAMPLE_TARGET_GAIN0 = 4, SAMPLE_
 struct VoiceArray { std::shared_ptr<const void> hold; uint64_t ptr = 0; uint32_t len = 0; };
 // What a per-voice call on voices [vb, vb + count) touches in one voice group: the node, its voices [b, e) there (group-relative), and
 // `at`, the index of voice b in the call's per-voice arrays.  snapshot() reports the value set for voice last(), the highest addressed.
-struct VoiceTarget { Group& g; Node& n; int b, e, at; int last() const { return at + e - b - 1; } };
 static bool voiceRangeOk(int vb, int count, int numVoices) { return vb >= 0 && count >= 0 && vb <= numVoices - count; }   // cannot overflow
 static VoiceArray seqArray(const std::shared_ptr<DeviceArray>& a) {
     return a ? VoiceArray{a, (uint64_t) (uintptr_t) a->d, (uint32_t) a->count} : VoiceArray{};
@@ -291,6 +291,8 @@ Engine::~Engine() {
     if (dDeliverDone_) cudaFree(dDeliverDone_);
     if (dResetPlan_) dfree(dResetPlan_);
     if (dResetCall_) dfree(dResetCall_);
+    if (dReadout_) dfree(dReadout_);
+    if (hReadout_) cudaFreeHost(hReadout_);
     if (wide_.dRows) dfree(wide_.dRows);
     if (wide_.dSegs) dfree(wide_.dSegs);
     if (wide_.dDst) dfree(wide_.dDst);
@@ -1327,6 +1329,27 @@ int Engine::voiceTargets(int32_t nodeId, int vb, int count, KindOk kindOk, const
         out.push_back(VoiceTarget{g, it->second, b - g.v0, e - g.v0, b - vb});
     }
     return rc::Ok;
+}
+
+// The checks of an array poll of one node (pollReadouts, processOfflineReadouts): the range, the node in every group, a meter or a snapshot,
+// and the same one of the two in every group (the arrays mean one thing).
+int Engine::readoutTargets(int32_t nodeId, int vb, int count, std::vector<VoiceTarget>& out) {
+    const int r = voiceTargets(nodeId, vb, count, [](NodeKind k) { return k == NodeKind::Meter || k == NodeKind::Snapshot; },
+                               "readouts are polled from meter and snapshot nodes", out);
+    if (r != rc::Ok) return r;
+    for (const VoiceTarget& t : out)
+        if (t.n.kind != out.front().n.kind) { out.clear(); return fail(rc::InvalidPropertyType, "the node is a meter in one voice group and a snapshot in another"); }
+    return rc::Ok;
+}
+
+std::string Engine::nodeType(int voice, int32_t nodeId) const {
+    Lock lk(mu_);
+    for (auto& g : groups_) {
+        if (voice < g->v0 || voice >= g->v0 + g->nv) continue;
+        auto it = g->nodes.find(nodeId);
+        return it == g->nodes.end() ? std::string() : it->second.typeName;
+    }
+    return std::string();
 }
 
 int Engine::setConstTable(const int32_t* nodeIds, int nProps, const float* values, int vb, int count) {
@@ -3125,6 +3148,27 @@ int Engine::processOfflineEvents(const float* const* in, size_t nIn, const float
     return offlineLoop(nIn ? in : nullptr, nIn, nIn ? inVoices : nullptr, mixOut, voicesOut, nOut, numSamples, chunkBlocks, sampleTime, &log);
 }
 
+int Engine::processOfflineReadouts(const float* const* in, size_t nIn, const float* inVoices, float* const* mixOut, float* voicesOut,
+                                   size_t nOut, size_t numSamples, size_t chunkBlocks, const int64_t* sampleTime,
+                                   const int32_t* nodeIds, int numNodes, int vb, int count, float* a, float* b, uint8_t* fresh) {
+    Lock lk(mu_);
+    if (numNodes < 1 || !nodeIds) return fail(rc::BadArgument, "processOfflineReadouts: no node to poll");
+    if (count < 1 || !a || !fresh) return fail(rc::BadArgument, "processOfflineReadouts: count < 1, or a or fresh is NULL");
+    ReadoutLog ro;
+    ro.nodes.assign(nodeIds, nodeIds + numNodes);
+    if (std::set<int32_t>(ro.nodes.begin(), ro.nodes.end()).size() != ro.nodes.size()) return fail(rc::BadArgument, "processOfflineReadouts: a node is listed twice");
+    ro.targets.resize((size_t) numNodes);
+    for (int j = 0; j < numNodes; ++j) {
+        const int r = readoutTargets(ro.nodes[j], vb, count, ro.targets[j]);
+        if (r != rc::Ok) return r;
+    }
+    const int r = offlineArgs(in, nIn, inVoices, voicesOut, nOut);
+    if (r != rc::Ok) return r;
+    ro.vb = vb; ro.count = count; ro.a = a; ro.b = b; ro.fresh = fresh;
+    ro.numBlocks = (numSamples + blockSize_ - 1) / blockSize_;
+    return offlineLoop(nIn ? in : nullptr, nIn, nIn ? inVoices : nullptr, mixOut, voicesOut, nOut, numSamples, chunkBlocks, sampleTime, nullptr, &ro);
+}
+
 // The chunk loop of both offline entry points (the engine lock is held).  Blocks are enqueued back to back with no host synchronisation in
 // between; chunk buffers of C blocks per row carry the inputs up and the outputs down, two of each on the device and two PINNED on the host.
 // The user's buffers are pageable and strided; a 2-D copy straight from or into them would be staged by the driver row by row,
@@ -3133,7 +3177,7 @@ int Engine::processOfflineEvents(const float* const* in, size_t nIn, const float
 // chunk k - 1's outputs while chunk k renders.  With an event log, K5 follows every block, the log travels down with the chunk's outputs
 // and its events are delivered once the chunk is scattered.
 int Engine::offlineLoop(const float* const* in, size_t nIn, const float* inVoices, float* const* mixOut, float* voicesOut,
-                        size_t nOut, size_t numSamples, size_t chunkBlocks, const int64_t* sampleTime, EventLog* log) {
+                        size_t nOut, size_t numSamples, size_t chunkBlocks, const int64_t* sampleTime, EventLog* log, ReadoutLog* ro) {
     dsetdev();
     const size_t bs = (size_t) blockSize_, numBlocks = (numSamples + bs - 1) / bs;
     if (numBlocks == 0) return rc::Ok;
@@ -3145,7 +3189,8 @@ int Engine::offlineLoop(const float* const* in, size_t nIn, const float* inVoice
         const int r = eventLogBegin(*log);
         if (r != rc::Ok) return r;
     }
-    const size_t blockFloats = std::max(maxRows * bs, log ? log->blockWords : 0);           // the largest chunk buffer, per block
+    const size_t logWords = log ? log->blockWords : ro ? ro->blockWords() : 0;               // a block's event log or readout records
+    const size_t blockFloats = std::max(maxRows * bs, logWords);                            // the largest chunk buffer, per block
     size_t C = chunkBlocks ? chunkBlocks : 8;
     while (C > 1 && blockFloats * C * sizeof(float) > ((size_t) 256 << 20)) C >>= 1;        // two chunk buffers of at most 256 MiB each
     if (C > numBlocks) C = numBlocks;
@@ -3157,7 +3202,7 @@ int Engine::offlineLoop(const float* const* in, size_t nIn, const float* inVoice
         return true;
     };
     if ((outRows && !ensure(offOut_, outRows * W)) || (inRows && !ensure(offIn_, inRows * W)) || (mixRows && !ensure(offMix_, mixRows * W)) ||
-        (log && log->blockWords && !ensure(offLog_, log->blockWords * C))) return rc::CudaError;
+        (logWords && !ensure(offLog_, logWords * C))) return rc::CudaError;
     cudaStream_t copyStream = nullptr, upStream = nullptr;
     cudaEvent_t rendered[2] = {nullptr, nullptr}, copied[2] = {nullptr, nullptr}, uploaded[2] = {nullptr, nullptr};
     int rcode = rc::Ok;
@@ -3193,6 +3238,9 @@ int Engine::offlineLoop(const float* const* in, size_t nIn, const float* inVoice
         for (size_t c = 0; c < mixRows; ++c)
             std::memcpy(mixOut[c] + s0, offMix_.pinned[pc.slot] + c * W, width * sizeof(float));
         if (log) rcode = eventLogReplay(*log, pc.slot, pc.chunk * C);
+        if (ro)
+            for (size_t k = 0; k < pc.blocks; ++k)
+                readoutScatter(*ro, reinterpret_cast<const uint32_t*>(offLog_.pinned[pc.slot]) + k * logWords, pc.chunk * C + k);
     };
     if (inRows && !stage(0)) rcode = rc::CudaError;
     BlockIO io;                                                                                 // block b: column b % C of its chunk's slot
@@ -3212,6 +3260,7 @@ int Engine::offlineLoop(const float* const* in, size_t nIn, const float* inVoice
         io.col = (int) (inChunk * bs);
         rcode = enqueueBlock(io);
         if (rcode == rc::Ok && log) rcode = eventLogBlock(*log, slot, inChunk);
+        if (rcode == rc::Ok && ro) rcode = readoutBlock(*ro, slot, inChunk);
         const bool lastOfChunk = inChunk + 1 == C || b + 1 == numBlocks;
         if (rcode == rc::Ok && lastOfChunk) {
             // the pinned buffers of this slot were scattered when chunk - 1 was enqueued (below), i.e. before these copies are issued
@@ -3220,6 +3269,7 @@ int Engine::offlineLoop(const float* const* in, size_t nIn, const float* inVoice
             if (outRows && !cuda(cudaMemcpyAsync(offOut_.pinned[slot], offOut_.dev[slot], outRows * W * sizeof(float), cudaMemcpyDeviceToHost, copyStream), "D2H offline chunk")) rcode = rc::CudaError;
             if (mixRows && !cuda(cudaMemcpyAsync(offMix_.pinned[slot], offMix_.dev[slot], mixRows * W * sizeof(float), cudaMemcpyDeviceToHost, copyStream), "D2H offline mix chunk")) rcode = rc::CudaError;
             if (log && log->used[slot] && !cuda(cudaMemcpyAsync(offLog_.pinned[slot], offLog_.dev[slot], log->used[slot] * sizeof(uint32_t), cudaMemcpyDeviceToHost, copyStream), "D2H offline event log")) rcode = rc::CudaError;
+            if (ro && !cuda(cudaMemcpyAsync(offLog_.pinned[slot], offLog_.dev[slot], (inChunk + 1) * logWords * sizeof(uint32_t), cudaMemcpyDeviceToHost, copyStream), "D2H offline readouts")) rcode = rc::CudaError;
             cudaEventRecord(copied[slot], copyStream);
             if (rcode == rc::Ok && inRows && chunk + 1 < numChunks && !stage(chunk + 1)) rcode = rc::CudaError;   // overlaps with this chunk's render
             Pending cur; cur.valid = true; cur.chunk = chunk; cur.blocks = inChunk + 1; cur.slot = slot;

@@ -47,7 +47,11 @@ struct DeviceArray {
     bool planOnly = false;
     ~DeviceArray();
 };
-struct VoiceArray; struct VoiceTarget;   // graph_host.cpp: the per-voice setters
+struct VoiceArray;   // graph_host.cpp: the per-voice setters
+struct Node;
+struct Group;
+// One voice group a per-voice call reaches: node n of group g, group-relative voices [b, e), which are voices [at, at + e - b) of the call.
+struct VoiceTarget { Group& g; Node& n; int b, e, at; int last() const { return at + e - b - 1; } };
 
 struct Inlet { int32_t source; int32_t channel; };
 
@@ -284,6 +288,18 @@ public:
     // Runtime::processQueuedEvents (Runtime.h:64,438-446): events of the voices [vb, ve); cb(type, event JSON, voice).
     typedef void (*EventFn)(const char* type, const char* json, int voice, void* user);
     int processQueuedEvents(int vb, int ve, EventFn cb, void* user);
+    // The poll of one meter / snapshot node over voices [vb, vb + count) into arrays (events_host.cpp): a / b / fresh[i] for voice vb + i,
+    // a and b written only where fresh[i] = 1 (meter: min / max; snapshot: the value, b unused; b may be null).  The side effects and the
+    // rules of processQueuedEvents for that node and those voices.  device: the arrays are device memory and the work is only enqueued;
+    // otherwise the stream is synchronised and the arrays are host memory.  Everything is checked before anything changes.
+    int pollReadouts(int32_t nodeId, int vb, int count, float* a, float* b, uint8_t* fresh, bool device);
+    // processOffline that also reads, after every block k, what pollReadouts(nodeIds[j], vb, count, ...) would read there, in node order:
+    // host arrays a / b / fresh [numNodes][numBlocks][count].  Event nodes not listed are not polled.
+    int processOfflineReadouts(const float* const* in, size_t nIn, const float* inVoices, float* const* mixOut, float* voicesOut,
+                               size_t nOut, size_t numSamples, size_t chunkBlocks, const int64_t* sampleTime,
+                               const int32_t* nodeIds, int numNodes, int vb, int count, float* a, float* b, uint8_t* fresh);
+    // The registered type name of node `nodeId` in the voice group containing `voice` ("" when there is none).
+    std::string nodeType(int voice, int32_t nodeId) const;
     void setCurrentTime(int64_t t) { Lock lk(mu_); sampleTime_ = t; }
     int64_t currentTime() const { Lock lk(mu_); return sampleTime_; }
     // Sum of the device durations (ms) of the K1 render kernels launched since the last call, measured with
@@ -389,12 +405,36 @@ private:
         std::vector<std::vector<PollItem>> blocks[2];
         size_t used[2] = {0, 0};
     };
+    // Array polls (pollReadouts, processOfflineReadouts).  A node's record holds [count] words of a, [count] of b, then count fresh bytes.
+    int readoutTargets(int32_t nodeId, int vb, int count, std::vector<VoiceTarget>& out);   // the checks of one node (graph_host.cpp)
+    static size_t readoutWords(int count) { return 2 * (size_t) count + ((size_t) count + 3) / 4; }
+    typedef std::set<std::pair<const Group*, int32_t>> PolledSet;   // (group, node) pairs a poll reaches
+    int readoutPolled(int vb, int ve, PolledSet& out);
+    // K5 items of one node's poll into device arrays a, b (null: not written), fresh; appended to `batch`, launched when full.  A group
+    // whose (group, node) pair is not in `polled` reports nothing and keeps its queue.
+    int readoutEnqueue(int32_t nodeId, const std::vector<VoiceTarget>& targets, const PolledSet& polled, uint32_t* a, uint32_t* b,
+                       uint8_t* fresh, EventLogBatch& batch);
+    int flushEventLog(EventLogBatch& batch);
+    struct ReadoutLog {
+        std::vector<int32_t> nodes;
+        std::vector<std::vector<VoiceTarget>> targets;
+        int vb = 0, count = 0;
+        float* a = nullptr; float* b = nullptr; uint8_t* fresh = nullptr;
+        size_t numBlocks = 0;
+        PolledSet polled;                 // the walk of the latest block
+        size_t blockWords() const { return nodes.size() * readoutWords(count); }
+    };
+    int readoutBlock(ReadoutLog& ro, int slot, size_t inChunk);
+    void readoutScatter(const ReadoutLog& ro, const uint32_t* rec, size_t block);   // one block's records into the caller's arrays
+    uint32_t* dReadout_ = nullptr; size_t readoutCap_ = 0;      // pollReadouts in host mode: the device staging buffer (words)
+    uint32_t* hReadout_ = nullptr; size_t readoutPinned_ = 0;   // and its pinned host copy
     int offlineArgs(const float* const* in, size_t nIn, const float* inVoices, float* voicesOut, size_t nOut);
     int eventLogBegin(EventLog& log);
     int eventLogBlock(EventLog& log, int slot, size_t inChunk);
     int eventLogReplay(EventLog& log, int slot, size_t firstBlock);
     int offlineLoop(const float* const* in, size_t nIn, const float* inVoices, float* const* mixOut, float* voicesOut,
-                    size_t nOut, size_t numSamples, size_t chunkBlocks, const int64_t* sampleTime, EventLog* log = nullptr);
+                    size_t nOut, size_t numSamples, size_t chunkBlocks, const int64_t* sampleTime, EventLog* log = nullptr,
+                    ReadoutLog* ro = nullptr);
     // Where a block's I/O lives: rows of `pitch` floats, the block in column `col` of each.  Device-resident calls pass the engine's own
     // buffers (pitch blockSize, column 0), offline blocks their chunk slots.
     struct BlockIO {

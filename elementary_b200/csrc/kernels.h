@@ -82,7 +82,10 @@ cudaError_t launch_mix_exchange(const PeerMix& pm, float* mix, int count, uint32
 //   EVLOG_CAPTURE  capture: log [3][n] words of state rows 2..4 (write position, read position, relay-ready flag), then [n][lim] floats:
 //                  the ring's samples [r, w) of each voice (at most lim); set the read position to w and clear the flag
 //   EVLOG_WINDOW   scope / fft: log [tile t0..t1)[channel < nch][size][L] floats, the ring window at read position r (no side effect)
-enum EventLogKind : int { EVLOG_ROWS = 0, EVLOG_CAPTURE = 1, EVLOG_WINDOW = 2 };
+//   EVLOG_READOUT  meter / snapshot as arrays (Engine::pollReadouts): fresh[i] = 1 where voice b + i's queue holds a readout (push count
+//                  mod 32 != 0), and then outA[i] = the bits of state row aRow, outB[i] (if not null) those of row 1; zero the push
+//                  count.  drain == 0 (the node is not under an active root): fresh[i] = 0 only, the rows are not read
+enum EventLogKind : int { EVLOG_ROWS = 0, EVLOG_CAPTURE = 1, EVLOG_WINDOW = 2, EVLOG_READOUT = 3 };
 struct EventLogItem {
     uint32_t* rows;           // the node's first state row (row j of voice v: rows[j * Vpad + v])
     const float* ring;        // capture: [tile][ringFloats][L]; scope / fft: [tile][ringCh][SCOPE_RING][L]
@@ -91,6 +94,10 @@ struct EventLogItem {
     uint32_t cap, lim, ringFloats;   // capture: ring capacity (a power of two), samples logged per voice at most, ring + scratch floats per lane
     uint32_t r, size;         // window: read position, window length
     int ringCh, nch, t0, t1;  // window: channels of the ring, channels logged, tiles
+    uint32_t* outA;           // readout: destinations of voices [b, b + n), compacted (outB may be null)
+    uint32_t* outB;
+    uint8_t* fresh;
+    int aRow, drain;          // readout: the state row `a` reads (meter 0 = min, snapshot 1 = value); drain the queue
 };
 constexpr int EVENT_LOG_BATCH = 32;   // items per launch (the batch travels as one kernel parameter)
 struct EventLogBatch { int n; EventLogItem item[EVENT_LOG_BATCH]; };

@@ -33,6 +33,7 @@ RETURN_CODES = {
 }
 
 FLAG_VOICE_IN, FLAG_VOICE_OUT, FLAG_MIX, FLAG_ALLREDUCE = 1, 2, 4, 8
+READOUT_DEVICE = 1      # elem_b200_poll_readouts: the arrays are device memory
 
 _lib = None
 
@@ -85,6 +86,14 @@ def load_library() -> C.CDLL:
     lib.elem_b200_process_offline_events.argtypes = [C.c_void_p, _f32pp, C.c_size_t, _f32p, _f32pp, _f32p, C.c_size_t, C.c_size_t, C.c_size_t,
                                                      C.c_void_p, C.c_int, C.c_int, BLOCK_EVENT_CB, C.c_void_p]
     lib.elem_b200_enqueue_block.argtypes = [C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_int]
+    lib.elem_b200_process_offline_readouts.restype = C.c_int
+    lib.elem_b200_process_offline_readouts.argtypes = [C.c_void_p, _f32pp, C.c_size_t, _f32p, _f32pp, _f32p, C.c_size_t, C.c_size_t, C.c_size_t,
+                                                       C.c_void_p, C.POINTER(C.c_int32), C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                                       C.c_void_p]
+    lib.elem_b200_poll_readouts.restype = C.c_int
+    lib.elem_b200_poll_readouts.argtypes = [C.c_void_p, C.c_int32, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
+    lib.elem_b200_node_type.restype = C.c_int
+    lib.elem_b200_node_type.argtypes = [C.c_void_p, C.c_int, C.c_int32, C.c_char_p, C.c_size_t]
     lib.elem_b200_peer_export.restype = C.c_int
     lib.elem_b200_peer_export.argtypes = [C.c_void_p, C.c_char_p]
     lib.elem_b200_peer_attach.restype = C.c_int
@@ -313,7 +322,8 @@ class Runtime:
     def process_offline(self, inputs: Optional[np.ndarray] = None, num_outputs: int = 1, num_samples: Optional[int] = None,
                         voice_inputs: Optional[np.ndarray] = None, want_mix: bool = True, want_voices: bool = False,
                         chunk_blocks: int = 0, sample_time: Optional[int] = None, on_event=None,
-                        event_voices: Optional[Sequence[int]] = None):
+                        event_voices: Optional[Sequence[int]] = None, readouts: Optional[Sequence[int]] = None,
+                        readout_voices: Optional[Sequence[int]] = None):
         """OfflineRenderer.process (js/packages/offline-renderer/index.ts:87-133): ceil(n / block_size) full blocks in one call, with
         ``inputs`` [n_in, n] broadcast to every voice or ``voice_inputs`` [voice, n_in, n] (zero past n), no host round trip per block.
         ``num_samples`` defaults to the inputs' length (one block without inputs).  ``sample_time``: as for :meth:`process`, for the
@@ -321,9 +331,16 @@ class Runtime:
 
         ``on_event(block, type, event_dict)``: every block's events, as :meth:`process_queued_events` (``voices`` = ``event_voices``)
         would report them right after the block (elem_b200_process_offline_events); called in block order before the call returns,
-        and it must not call into this runtime.  An exception it raises is re-raised once the call has returned."""
+        and it must not call into this runtime.  An exception it raises is re-raised once the call has returned.
+
+        ``readouts``: meter / snapshot node ids whose readouts are read after every block as :meth:`poll_readouts` would read them,
+        polled in the order given, for the voices ``readout_voices`` = (begin, end) (default: all); no other event node is polled
+        (elem_b200_process_offline_readouts).  The call then returns a third element, ``{node_id: {...}}`` with the arrays of
+        :meth:`poll_readouts` shaped [blocks, voices].  Not together with ``on_event``."""
         if inputs is not None and voice_inputs is not None:
             raise ValueError("process_offline: give inputs or voice_inputs, not both")
+        if readouts is not None and on_event is not None:
+            raise ValueError("process_offline: give readouts or on_event, not both")
         src = inputs if inputs is not None else voice_inputs
         keep = None if src is None else np.ascontiguousarray(np.asarray(src, dtype=np.float32))
         n = int(num_samples if num_samples is not None else (keep.shape[-1] if keep is not None else self.block_size))
@@ -342,6 +359,16 @@ class Runtime:
         mix_ptrs = (_f32p * max(1, num_outputs))(*[mix[i].ctypes.data_as(_f32p) for i in range(num_outputs)]) if want_mix else None
         user = None if sample_time is None else C.byref(C.c_int64(int(sample_time)))
         ov_ptr = ov.ctypes.data_as(_f32p) if ov is not None else None
+        if readouts is not None:
+            ids = np.ascontiguousarray(np.asarray(readouts, dtype=np.int32).reshape(-1))
+            vb, ve = (0, self.num_voices) if readout_voices is None else (int(readout_voices[0]), int(readout_voices[1]))
+            shape = (ids.size, -(-n // self.block_size), max(0, ve - vb))
+            a, b, fresh = np.zeros(shape, np.float32), np.zeros(shape, np.float32), np.zeros(shape, np.uint8)
+            rc = self._lib.elem_b200_process_offline_readouts(self._h, in_ptrs, n_in, vin_ptr, mix_ptrs, ov_ptr, num_outputs, n,
+                                                              int(chunk_blocks), user, ids.ctypes.data_as(C.POINTER(C.c_int32)), ids.size,
+                                                              vb, ve - vb, a.ctypes.data, b.ctypes.data, fresh.ctypes.data)
+            self._check(rc, "process_offline")
+            return mix, ov, {int(i): self._readout_dict(int(i), vb, a[j], b[j], fresh[j]) for j, i in enumerate(ids)}
         if on_event is None:
             rc = self._lib.elem_b200_process_offline(self._h, in_ptrs, n_in, vin_ptr, mix_ptrs, ov_ptr, num_outputs, n, int(chunk_blocks), user)
             self._check(rc, "process_offline")
@@ -457,6 +484,36 @@ class Runtime:
         vb, ve = (0, -1) if voices is None else (int(voices[0]), int(voices[1]))
         self._check(self._lib.elem_b200_process_queued_events_range(self._h, vb, ve, cb, None), "process_queued_events")
         return events
+
+    def poll_readouts(self, node_id: int, voices: Optional[Sequence[int]] = None) -> dict:
+        """The poll of one meter or snapshot node over ``voices`` = (begin, end) (default: all) into arrays, index i = voice begin + i
+        (elem_b200_poll_readouts): ``{"min", "max", "fresh"}`` for a meter, ``{"data", "fresh"}`` for a snapshot.  ``fresh[i]`` is 1 where
+        :meth:`process_queued_events` would have reported an event for that voice, with the same side effects; elsewhere the values are 0."""
+        vb, ve = (0, self.num_voices) if voices is None else (int(voices[0]), int(voices[1]))
+        n = max(0, ve - vb)
+        a, b, fresh = np.zeros(n, np.float32), np.zeros(n, np.float32), np.zeros(n, np.uint8)
+        rc = self._lib.elem_b200_poll_readouts(self._h, int(node_id), vb, ve - vb, a.ctypes.data, b.ctypes.data, fresh.ctypes.data, 0)
+        self._check(rc, "poll_readouts")
+        return self._readout_dict(int(node_id), vb, a, b, fresh)
+
+    def poll_readouts_device(self, node_id: int, a_ptr: int, b_ptr: Optional[int], fresh_ptr: int,
+                             voices: Optional[Sequence[int]] = None) -> None:
+        """:meth:`poll_readouts` into device memory (float32 ``a`` and ``b``, uint8 ``fresh``, e.g. ``tensor.data_ptr()``; ``b_ptr`` may
+        be None): enqueued on the runtime's stream, no synchronisation.  ``a`` is the min or the value, ``b`` the max."""
+        vb, ve = (0, self.num_voices) if voices is None else (int(voices[0]), int(voices[1]))
+        rc = self._lib.elem_b200_poll_readouts(self._h, int(node_id), vb, ve - vb, a_ptr or None, b_ptr or None, fresh_ptr or None, READOUT_DEVICE)
+        self._check(rc, "poll_readouts_device")
+
+    def node_type(self, node_id: int, voice: int = 0) -> Optional[str]:
+        """The type name of ``node_id`` in the voice group containing ``voice``, or None."""
+        buf = C.create_string_buffer(64)
+        n = self._lib.elem_b200_node_type(self._h, int(voice), int(node_id), buf, len(buf))
+        return buf.value.decode() if n else None
+
+    def _readout_dict(self, node_id, voice, a, b, fresh) -> dict:
+        if self.node_type(node_id, voice) == "snapshot":
+            return {"data": a, "fresh": fresh}
+        return {"min": a, "max": b, "fresh": fresh}
 
     # -- introspection ------------------------------------------------------------------------------------------
     def set_option(self, key: str, value: float) -> None:

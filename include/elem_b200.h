@@ -197,6 +197,24 @@ int elem_b200_process_offline_events(elem_b200_runtime* rt, const float* const* 
                                      size_t chunkBlocks, void* userData, int voiceBegin, int voiceEnd,
                                      elem_b200_block_event_cb cb, void* user);
 
+/* elem_b200_process_offline with every block's meter / snapshot readouts as arrays (see elem_b200_poll_readouts) instead of events.
+ * Arguments, blocks, chunks, sample clock, outputs and their errors are those of elem_b200_process_offline, and the audio is bit for bit
+ * what it returns.
+ * READOUTS: a, b, fresh are host arrays [numNodes][numBlocks][count], numBlocks = ceil(numSamples / blockSize).  Entry [j][k][i] is what
+ *   elem_b200_poll_readouts(rt, nodeIds[j], voiceBegin, count, ...) would write for voice voiceBegin + i right after the k-th of the
+ *   equivalent elem_b200_process calls, the listed nodes polled in the order given: a and b only where fresh is 1; b may be NULL.
+ *   After each block a K5 launch writes every listed node's readouts into a record that travels down with the chunk's outputs; the chunk
+ *   size shrinks so that two of these logs stay within 256 MiB each.  Event nodes not listed are not polled: their queues end as un-polled
+ *   elem_b200_process calls leave them.  The engine lock is held for the whole call.
+ * Returns, before rendering anything, what elem_b200_process_offline returns, and -2 for numNodes < 1, a node id listed twice, count < 1,
+ *   a NULL `a` or `fresh` or a voice range outside [0, numVoices); NodeNotFound (2) and InvalidPropertyType (5) per node as
+ *   elem_b200_poll_readouts returns them.  No reference method: the reference has no voice axis. */
+int elem_b200_process_offline_readouts(elem_b200_runtime* rt, const float* const* in, size_t nIn, const float* inVoices,
+                                       float* const* mixOut, float* voicesOut, size_t nOut, size_t numSamples,
+                                       size_t chunkBlocks, void* userData,
+                                       const int32_t* nodeIds, int numNodes, int voiceBegin, int count,
+                                       float* a, float* b, uint8_t* fresh);
+
 /* Device-resident stepping for throughput measurement and pipelines that keep audio in HBM: enqueue one block
  * on the engine's stream (no host copies, no synchronisation).  flags: 1 = read per-voice inputs from
  * elem_b200_voice_in_device(), 2 = materialise per-voice outputs, 4 = produce the mix bus, 8 = (with 4, after
@@ -257,6 +275,26 @@ void elem_b200_process_queued_events(elem_b200_runtime* rt, elem_b200_event_cb c
  * voice), so a poll that reaches a group consumes that window for the whole group. */
 int elem_b200_process_queued_events_range(elem_b200_runtime* rt, int voiceBegin, int voiceEnd, elem_b200_event_cb cb, void* user);
 
+/* The poll of one `meter` or `snapshot` node over the voices [voiceBegin, voiceBegin + count), into arrays instead of one JSON event per
+ * voice; index i is voice voiceBegin + i, across every voice group of the range.
+ *   meter     a[i] = min, b[i] = max;   snapshot  a[i] = the latched value, b is never written.  b may be NULL.
+ *   fresh[i]  1 exactly when elem_b200_process_queued_events_range over the same voices, called now, would deliver an event of this node
+ *             for that voice (the sequence the last process() used, an active root, a queue not pushed a multiple of 32 times since its
+ *             last drain); a[i] and b[i] are written only then, as the float32 bits of the readout (a non-finite value too, where the
+ *             JSON text has null).
+ * Side effects: those of that poll on this node and these voices — the queues under an active root are drained — and nothing else, so
+ * a later JSON poll sees nothing from the voices drained here, and the reverse.
+ * flags 0: host arrays; the call synchronises the render stream.  ELEM_B200_READOUT_DEVICE: device arrays on the runtime's device; the
+ * work is enqueued on the runtime's stream and the call returns without synchronising (order reads after it with elem_b200_synchronize
+ * or through elem_b200_set_stream), so a loop of elem_b200_enqueue_block + this call has no host round trip per block.
+ * Returns -2 for a voice range out of bounds, count < 0, or a NULL `a` or `fresh` with count > 0; NodeNotFound (2) when a voice group
+ * in the range lacks the node; InvalidPropertyType (5) when it is not a meter or snapshot (or a meter in one group and a snapshot in
+ * another); 0 and nothing launched for count == 0; -1 on a plan-only runtime.  All of it is checked before anything changes.  A
+ * control-thread call, like elem_b200_process_queued_events.  No reference method: the reference has no voice axis. */
+#define ELEM_B200_READOUT_DEVICE 1
+int elem_b200_poll_readouts(elem_b200_runtime* rt, int32_t nodeId, int voiceBegin, int count,
+                            float* a, float* b, uint8_t* fresh, int flags);
+
 /* Tuning and introspection (no reference equivalent).  Keys: "tile_width" (1..32 voices per warp, 0 = auto), "warps_per_cta",
  * "target_tiles", "niter" (sample-tile variant: 4 = 128-sample one-voice tiles), "batch_groups", "fuse_chains",
  * "specialize" (per-program NVRTC kernels: 0 off, 1 compile in the background while the interpreter serves, 2 wait at COMMIT),
@@ -282,6 +320,10 @@ int elem_b200_has_node_type(elem_b200_runtime* rt, const char* type);
  * {"0x<node id as 8 hex digits>": {<props>}, ...} (nodeIdToHex, Types.h:16-27; props as they were last set, GraphNode.h:60-64,130).
  * Returns the bytes needed including the terminating NUL; writes at most cap. */
 int elem_b200_snapshot(elem_b200_runtime* rt, int voice, char* buf, size_t cap);
+/* The type name of node `nodeId` ("meter", "snapshot", ...) in the voice group containing `voice` — what snapshot() does not carry, and
+ * what tells a caller of elem_b200_poll_readouts whether `a` / `b` are min / max or a snapshot's value.  Writes up to `cap` bytes
+ * including the terminating NUL, returns the name's length + 1, or 0 when that group has no such node.  No reference method. */
+int elem_b200_node_type(elem_b200_runtime* rt, int voice, int32_t nodeId, char* buf, size_t cap);
 
 /* JSON description of voice groups and compiled programs; returns bytes needed.  "steady": the next block of the same shape relaunches
  * cached work without walking the groups.  Per group, "mix_channels": the non-negative root channels of the program the last block
